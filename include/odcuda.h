@@ -593,6 +593,23 @@ int od_coastline(od_ctx* ctx, const od_coast_args* a);
 int od_store_previous(od_ctx* ctx, int64_t n, const double* d_lon, const double* d_lat, const int32_t* d_ids, int32_t id_base,
                       int64_t n_total, float* d_prev_lon, float* d_prev_lat);
 
+/* ---- a varying sea surface height (csrc/od_sealevel.cuh) ------------------------------------------------------
+ * od_store_previous_env is update_previous_state (basemodel/__init__.py:642-657) for one float32 environment variable
+ * (sea_surface_height): d_prev[i] = the stored value of element i -- the present one for an element released this step --
+ * then d_store[ID - id_base] = d_present.  d_store is [n_total], NaN at the start of the run.  d_age (age_seconds after
+ * increase_age_and_retire, float32 / float64 by age_f64) is given on steps that released elements, else NULL; elements of
+ * age == dt are the newly seeded ones, whose present values the reference also writes at their POSITIONS in the store --
+ * reproduced.  Two launches.
+ * od_vertical_advection_corrected is OceanDrift.vertical_advection with drift:vertical_advection_correction
+ * (oceandrift.py:325-350), in place on d_z (float32 / float64 by z_f64): w -= (delta_zeta / dt) * (z + H) / H with
+ * delta_zeta = ssh - ssh_prev, H = ssh + sea floor depth (d_floor, or floor_const when NULL), then z = min(0, z + moving*w*dt)
+ * for z < 0 (z <= 0 when at_surface); NumPy's dtypes and operation order. */
+int od_store_previous_env(od_ctx* ctx, int64_t n, const float* d_present, const int32_t* d_ids, const void* d_age, int32_t age_f64,
+                          double dt, int32_t id_base, int64_t n_total, float* d_store, float* d_prev);
+int od_vertical_advection_corrected(od_ctx* ctx, int64_t n, void* d_z, int32_t z_f64, const float* d_w, const float* d_ssh,
+                                    const float* d_ssh_prev, const float* d_floor, float floor_const, const int32_t* d_moving,
+                                    int32_t at_surface, double dt);
+
 /* ---- particle exchange of the spatial-tile mode --------------------------------------------------------------
  * BASELINE configs[2]: every rank owns one longitude strip of the domain (and holds only that part of the forcing, plus a halo);
  * after a step the elements that left their strip travel to the new owner in ONE all-to-all.  od_pack_by_owner groups the

@@ -205,6 +205,9 @@ SYMBOLS = {
     'od_bookkeeping': (C.c_int, [_P, C.POINTER(BookkeepArgs)]),
     'od_coastline': (C.c_int, [_P, C.POINTER(CoastArgs)]),
     'od_store_previous': (C.c_int, [_P, C.c_int64, _P, _P, _P, C.c_int32, C.c_int64, _P, _P]),
+    'od_store_previous_env': (C.c_int, [_P, C.c_int64, _P, _P, _P, C.c_int32, C.c_double, C.c_int32, C.c_int64, _P, _P]),
+    'od_vertical_advection_corrected': (C.c_int, [_P, C.c_int64, _P, C.c_int32, _P, _P, _P, _P, C.c_float, _P, C.c_int32,
+                                                  C.c_double]),
     'od_pack_by_owner': (C.c_int, [_P, C.POINTER(PackArgs)]),
     'od_unpack_records': (C.c_int, [_P, C.c_int64, _P, C.c_int32, C.POINTER(_P), C.POINTER(C.c_int32), C.c_int32]),
     'od_sort_by_cell': (C.c_int, [_P, C.c_int, C.c_int64, _P, _P, _P, _P]),

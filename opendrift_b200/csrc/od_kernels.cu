@@ -23,6 +23,7 @@
 #include "od_analytic.cuh"
 #include "od_history.cuh"
 #include "od_bookkeep.cuh"
+#include "od_sealevel.cuh"
 #include "od_ctx.cuh"
 
 extern "C" int od_abi_version(void) { return OD_ABI_VERSION; }
@@ -671,6 +672,21 @@ __global__ void __launch_bounds__(256) store_previous_kernel(int64_t n, const do
                                                              float* __restrict__ prev_lon, float* __restrict__ prev_lat) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i < n) store_previous_one(i, lon, lat, ids, id_base, n_total, prev_lon, prev_lat);
+}
+
+__global__ void __launch_bounds__(256) store_prev_gather_kernel(const StorePrevParams p) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < p.n) store_prev_gather_one(p, i);
+}
+
+__global__ void __launch_bounds__(256) store_prev_scatter_kernel(const StorePrevParams p) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < p.n) store_prev_scatter_one(p, i);
+}
+
+__global__ void __launch_bounds__(256) vadv_corrected_kernel(const VadvCorrParams p) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < p.n) vadv_corrected_one(p, i);
 }
 
 __global__ void __launch_bounds__(OD_BLOCK) geod_fwd_kernel(int64_t n, double* __restrict__ lon, double* __restrict__ lat,
@@ -1626,6 +1642,41 @@ extern "C" int od_store_previous(od_ctx* ctx, int64_t n, const double* lon, cons
     if (n == 0) return OD_OK;
     CK(cudaSetDevice(ctx->device));
     store_previous_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(n, lon, lat, ids, id_base, n_total, prev_lon, prev_lat);
+    CK(cudaGetLastError());
+    ctx->launches++;
+    return OD_OK;
+}
+
+extern "C" int od_store_previous_env(od_ctx* ctx, int64_t n, const float* present, const int32_t* ids, const void* age, int32_t age_f64,
+                                     double dt, int32_t id_base, int64_t n_total, float* store, float* prev) {
+    if (!ctx || n < 0 || n_total < 0 || (n > 0 && (!present || !ids || !store || !prev)))
+        return fail(ctx, OD_ERR_ARG, "od_store_previous_env: bad arguments");
+    if (n == 0) return OD_OK;
+    CK(cudaSetDevice(ctx->device));
+    StorePrevParams p;
+    p.n = n; p.present = present; p.ids = ids; p.age = age; p.store = store; p.prev = prev; p.n_total = n_total; p.id_base = id_base;
+    p.age_f64 = age_f64; p.dt = dt;
+    const unsigned blocks = (unsigned)((n + 255) / 256);
+    // gather (and the positional writes) must be complete before the scatter overwrites the slots it reads: two launches
+    store_prev_gather_kernel<<<blocks, 256, 0, ctx->stream>>>(p);
+    CK(cudaGetLastError());
+    store_prev_scatter_kernel<<<blocks, 256, 0, ctx->stream>>>(p);
+    CK(cudaGetLastError());
+    ctx->launches += 2;
+    return OD_OK;
+}
+
+extern "C" int od_vertical_advection_corrected(od_ctx* ctx, int64_t n, void* z, int32_t z_f64, const float* w, const float* ssh,
+                                               const float* ssh_prev, const float* floor, float floor_const, const int32_t* moving,
+                                               int32_t at_surface, double dt) {
+    if (!ctx || n < 0 || (n > 0 && (!z || !w || !ssh || !ssh_prev || !moving)))
+        return fail(ctx, OD_ERR_ARG, "od_vertical_advection_corrected: bad arguments");
+    if (n == 0) return OD_OK;
+    CK(cudaSetDevice(ctx->device));
+    VadvCorrParams p;
+    p.n = n; p.z = z; p.w = w; p.ssh = ssh; p.ssh_prev = ssh_prev; p.floor = floor; p.moving = moving; p.floor_const = floor_const;
+    p.z_f64 = z_f64; p.at_surface = at_surface; p.dt = dt;
+    vadv_corrected_kernel<<<(unsigned)((n + 255) / 256), 256, 0, ctx->stream>>>(p);
     CK(cudaGetLastError());
     ctx->launches++;
     return OD_OK;

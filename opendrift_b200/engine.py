@@ -570,6 +570,33 @@ class Engine:
         self._check(self.lib.od_store_previous(self.ctx, lon.numel(), _ptr(lon), _ptr(lat), _ptr(ids), int(id_base), prev_lon.numel(),
                                                _ptr(prev_lon), _ptr(prev_lat)))
 
+    def store_previous_env(self, present, ids, age, dt, id_base, store):
+        """update_previous_state (:642-657) for one float32 environment variable: returns the previous values of the active
+        elements and stores the present ones into `store` ([n_total] float32, keyed by ID - id_base).  age: age_seconds
+        on a step that released elements, else None."""
+        torch = self.torch
+        assert present.dtype == torch.float32 and ids.dtype == torch.int32 and store.dtype == torch.float32
+        prev = self.empty(present.numel(), torch.float32)
+        age_f64 = 0
+        if age is not None:
+            assert age.dtype in (torch.float32, torch.float64)
+            age_f64 = 1 if age.dtype == torch.float64 else 0
+        self._check(self.lib.od_store_previous_env(self.ctx, present.numel(), _ptr(present), _ptr(ids), _ptr(age), age_f64, float(dt),
+                                                   int(id_base), store.numel(), _ptr(store), _ptr(prev)))
+        return prev
+
+    def vertical_advection_corrected(self, z, w, ssh, ssh_prev, floor, moving, at_surface, dt):
+        """OceanDrift.vertical_advection with drift:vertical_advection_correction (oceandrift.py:325-350), in place on z.
+        floor: float32 tensor or a number."""
+        torch = self.torch
+        assert z.dtype in (torch.float32, torch.float64) and moving.dtype == torch.int32
+        assert w.dtype == ssh.dtype == ssh_prev.dtype == torch.float32
+        fl, fc = (floor, 0.0) if hasattr(floor, 'data_ptr') else (None, float(floor))
+        assert fl is None or fl.dtype == torch.float32
+        self._check(self.lib.od_vertical_advection_corrected(self.ctx, z.numel(), _ptr(z), 1 if z.dtype == torch.float64 else 0, _ptr(w),
+                                                             _ptr(ssh), _ptr(ssh_prev), _ptr(fl), fc, _ptr(moving),
+                                                             1 if at_surface else 0, float(dt)))
+
     def geod_fwd(self, lon, lat, az, dist):
         self._check(self.lib.od_geod_fwd(self.ctx, lon.numel(), _ptr(lon), _ptr(lat), _ptr(az), _ptr(dist)))
 

@@ -57,6 +57,16 @@ class EnvironmentView:
     def __contains__(self, name):
         return name in self._t or name in self._h
 
+    def permute(self, perm, engine):
+        """Re-order the rows as the element arrays were re-ordered (row k <- row perm[k])."""
+        t, h = object.__getattribute__(self, '_t'), object.__getattribute__(self, '_h')
+        for k in list(t):
+            t[k] = engine.permute(perm, t[k]) if t[k].dim() == 1 else t[k][perm.long()]
+        if h:
+            ph = perm.cpu().numpy()
+            for k in list(h):
+                h[k] = h[k][ph]
+
     def select(self, keep):
         """Keep the rows of the elements selected by the boolean device tensor `keep`."""
         t, h = object.__getattribute__(self, '_t'), object.__getattribute__(self, '_h')
@@ -406,7 +416,8 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
         pre = getattr(self, '_noise0', None)
         view = getattr(self, '_env_view', None)
         keep = keep_dev = None
-        if pre or view is not None:
+        ssh = getattr(self, '_ssh_now', None)
+        if pre or view is not None or ssh is not None:
             keep_dev = self.elements.dev('status') == 0
             if pre:
                 keep = keep_dev.cpu().numpy()
@@ -416,6 +427,8 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
                 pre[k] = [a[keep] for a in pre[k]]
         if view is not None and removed is not None:       # self.environment = self.environment[~indices] (:1812-1813)
             view.select(keep_dev)
+        if ssh is not None and removed is not None:
+            self._ssh_now = ssh[keep_dev]
         if removed is None:
             return
         tmp = self.ElementType(**{k: v for k, v in removed.items()})
@@ -581,6 +594,9 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
         eng, el, torch = self.engine, self.elements, self.engine.torch
         cats = self.status_categories
         mask = self._start_of_step_sample('land_binary_mask')
+        if self._vertical_advection_correction():
+            # an element with an undefined depth is not covered by the mask reader (see report_missing_variables): NaN, no action
+            mask = torch.where(torch.isnan(self._z_for_sampling()), torch.full_like(mask, float('nan')), mask)
         self._coast_moved = False
         if self._coast == 'previous' and not final and bool((mask == 1).any()):
             # Elements on land go back to where they were, but update() still sees the environment sampled where they are now
@@ -630,11 +646,21 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
         top of the loop.  Costs nothing with the default configuration (every variable of the stock recipes has a fallback value);
         otherwise those variables are sampled here, before deactivate_outside as in the reference."""
         may_miss = self._variables_that_may_miss()
-        if not may_miss or self.num_elements_active() == 0:
+        # No reader covers an element with an undefined depth: the reference's coverage test is zmin <= z <= zmax for gridded, 2-D
+        # and constant readers alike (readers/basereader/variables.py:241-251), so a variable without a fallback value is missing
+        # there, wherever it comes from (the device samplers of 2-D fields do not look at z).  Undefined depths come from
+        # drift:vertical_advection_correction: an element without a previous sea surface height (update_previous_state)
+        nan_z = self._vertical_advection_correction() and any(self.env.fallback(v) is None for v in getattr(self, '_env_variables', ()))
+        if (not may_miss and not nan_z) or self.num_elements_active() == 0:
             return
         el, torch = self.elements, self.engine.torch
-        _, missing = self.env.device_environment(may_miss, self.time, el.dev('lon', torch.float64), el.dev('lat', torch.float64),
-                                                 self._z_truncated(), pos_f32=el.positions_f32)
+        missing = None
+        if may_miss:
+            _, missing = self.env.device_environment(may_miss, self.time, el.dev('lon', torch.float64), el.dev('lat', torch.float64),
+                                                     self._z_truncated(), pos_f32=el.positions_f32)
+        if nan_z:
+            undefined = torch.isnan(self._z_for_sampling())
+            missing = undefined if missing is None else (missing | undefined)
         self._deactivate_missing(missing)
 
     def _deactivate_missing(self, missing):
@@ -657,12 +683,88 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
                 self.status_categories.append('outside')
 
     def update_previous_state(self):
-        """:642-669 for lon / lat (the element properties the reference stores when a coastline action may move elements back)."""
-        if not getattr(self, '_store_previous', False) or self.num_elements_active() == 0:
+        """:642-669 for lon / lat (the element properties the reference stores when a coastline action may move elements back) and
+        for sea_surface_height (the environment variable OceanDrift stores while vertical advection is on)."""
+        if self.num_elements_active() == 0:
             return
         el, torch = self.elements, self.engine.torch
+        if getattr(self, '_ssh_store', None) is not None:
+            age = None
+            if getattr(self, '_newly_seeded', False):              # newly_seeded_IDs is not None (:645-653)
+                age = el.dev('age_seconds')
+                if age.dtype not in (torch.float32, torch.float64):
+                    age = age.to(torch.float64)
+            self._ssh_prev = self.engine.store_previous_env(self._ssh_tensor(), el.dev('ID', torch.int32), age,
+                                                            self.time_step.total_seconds(), self._id_base, self._ssh_store)
+            self.environment_previous = EnvironmentView({'sea_surface_height': self._ssh_prev})
+        if not getattr(self, '_store_previous', False):
+            return
         self.engine.store_previous(el.dev('lon', torch.float64), el.dev('lat', torch.float64), el.dev('ID', torch.int32), self._id_base,
                                    self._prev_lon, self._prev_lat)
+
+    # -- sea surface height (the water column is sea_floor_depth_below_sea_level + sea_surface_height) -----------------------
+    def _vertical_advection_correction(self):
+        return 'drift:vertical_advection_correction' in self._config and bool(self.get_config('drift:vertical_advection_correction'))
+
+    def _ssh_reads(self):
+        """Does anything in this run read the sea surface height per element?  (Overridden by OceanDrift.)"""
+        return bool(self.env.priority_list.get('sea_floor_depth_below_sea_level'))
+
+    def _setup_sea_level(self):
+        """The previous-step store of sea_surface_height (required_variables store_previous_if, :1917-1924, :2162-2163: float32 per
+        trajectory, NaN at the start) runs when its condition holds and the value can change -- a reader, a non-zero constant --
+        or drift:vertical_advection_correction reads it.  A reader is sampled at the top of every step that something reads it in."""
+        self._ssh_store = self._ssh_now = self._ssh_prev = None
+        self.environment_previous = None
+        self._ssh_sample_at_top = False
+        spec = self.required_variables.get('sea_surface_height')
+        if spec is None:
+            return
+        reader = bool(self.env.priority_list.get('sea_surface_height'))
+        varies = reader or (self.env.constant('sea_surface_height') or 0) != 0
+        cond = spec.get('store_previous_if')
+        if cond is not None:
+            key, op, val = cond
+            cur = self.get_config(key)
+            if ((op == 'is' and cur is val) or (op == 'in' and cur in val)) and (varies or self._vertical_advection_correction()):
+                torch = self.engine.torch
+                self._ssh_store = torch.full((len(self._release_rank),), float('nan'), dtype=torch.float32, device=self.engine.device)
+        self._ssh_sample_at_top = reader and (self._ssh_store is not None or self._ssh_reads())
+
+    def _sea_surface_height(self):
+        """sea_surface_height at the elements at the start of the step: a float when no reader provides it (constant, else
+        fallback), else the float32 device tensor."""
+        if 'sea_surface_height' not in self.required_variables:
+            return 0.0
+        if not self.env.priority_list.get('sea_surface_height'):
+            c = self.env.constant('sea_surface_height')
+            if c is None:
+                c = self.env.fallback('sea_surface_height')
+            return float(c or 0.0)
+        if getattr(self, '_ssh_now', None) is None:
+            self._ssh_now = self._start_of_step_sample('sea_surface_height')
+        return self._ssh_now
+
+    def _ssh_tensor(self):
+        s = self._sea_surface_height()
+        if hasattr(s, 'data_ptr'):
+            return s
+        torch = self.engine.torch
+        return torch.full((self.num_elements_active(),), float(np.float32(s)), dtype=torch.float32, device=self.engine.device)
+
+    def _water_column(self, floor, tensor=False):
+        """(sea floor, sea surface height) to hand to the kernels that compare depths with -(floor + ssh): with a per-element
+        sea surface height, (floor + ssh as one float32 tensor -- NumPy's float32 sum --, 0.0); else (floor, the scalar ssh).
+        tensor=True: a float32 tensor for the column whenever the sea surface height is not zero."""
+        ssh = self._sea_surface_height()
+        if not hasattr(ssh, 'data_ptr') and (ssh == 0 or not tensor):
+            return floor, ssh
+        torch = self.engine.torch
+        if not hasattr(ssh, 'data_ptr'):
+            ssh = self._ssh_tensor()
+        if not hasattr(floor, 'data_ptr'):
+            floor = torch.full_like(ssh, float(np.float32(floor)))
+        return floor + ssh, 0.0
 
     def interact_with_seafloor(self):
         """:748-783 -- elements below the sea floor (sea_floor_depth_below_sea_level from a reader + sea_surface_height) are lifted
@@ -673,9 +775,7 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
         if action == 'none':
             return
         eng, el, torch = self.engine, self.elements, self.engine.torch
-        floor = self._start_of_step_sample('sea_floor_depth_below_sea_level')
-        ssh = float(self.env.constant('sea_surface_height') or self.env.fallback('sea_surface_height') or 0.0) \
-            if 'sea_surface_height' in self.required_variables else 0.0
+        floor, ssh = self._water_column(self._start_of_step_sample('sea_floor_depth_below_sea_level'))
         if action == 'previous':
             # elements below the floor go back to the horizontal position of the previous step, their depth stays (:775-783)
             lon, lat = el.dev('lon', torch.float64), el.dev('lat', torch.float64)
@@ -911,12 +1011,9 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
             raise NotImplementedError('file export is outside the GPU hot path; read o.history / o.elements')
         if self.num_elements_scheduled() == 0:
             raise ValueError('Please seed elements before starting a run.')
-        for key in ('drift:water_column_stretching', 'drift:use_tabularised_stokes_drift', 'drift:vertical_advection_correction',
-                    'vertical_mixing:TSprofiles'):
+        for key in ('drift:water_column_stretching', 'drift:use_tabularised_stokes_drift', 'vertical_mixing:TSprofiles'):
             if key in self._config and self.get_config(key):
                 raise NotImplementedError('%s = True is not on the GPU path' % key)
-        if self.env.priority_list.get('sea_surface_height') or (self.env.constant('sea_surface_height') or 0) != 0:
-            raise NotImplementedError('a varying sea_surface_height (sea-level correction of depths) is not on the GPU path')
         from .. import _lib
         self.engine.math_mode = {'series': _lib.OD_MATH_SERIES, 'exact': _lib.OD_MATH_EXACT,
                                  'fast': _lib.OD_MATH_FAST}[self.get_config('gpu:arithmetic')]
@@ -984,6 +1081,10 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
         if getattr(eng, 'dist', None) is None and self.get_config('gpu:distributed') and hasattr(eng, 'enable_distributed'):
             eng.enable_distributed()
         self._dist = getattr(eng, 'dist', None)
+        if self._dist is not None and self._vertical_advection_correction():
+            # the reference's previous-step store writes newly released elements at their positions in the whole element array
+            # (update_previous_state :651-653); a shard sees only its own positions
+            raise NotImplementedError('drift:vertical_advection_correction = True is not on the distributed GPU path')
         self.shard = None
         if self._dist is not None and self.get_config('gpu:shard') == 'index':
             n_all = int(self.num_elements_total())
@@ -1000,6 +1101,7 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
         self.steps_calculation = 0
         self._maybe_deactivated = False
         self._setup_coastline()
+        self._setup_sea_level()
         if self.env.has_ensembles():
             ok = getattr(self, '_ensemble_variables', ())
             bad = [v for v in self.env.priority_list if self.env.has_ensembles([v]) and v not in ok]
@@ -1036,6 +1138,10 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
                 self._env_view = None
                 if self._has_subblock_readers:
                     self._cover_elements_with_blocks()
+                self._ssh_now = None
+                if self._ssh_sample_at_top:
+                    # sampled with the step's environment, before anything moves the elements (:2238-2256)
+                    self._ssh_now = self._start_of_step_sample('sea_surface_height')
                 self._predraw_step_uncertainty()
                 # deactivate_outside -> interact_with_seafloor -> state_to_buffer -> increase_age_and_retire (:2249-2260)
                 col, only_deact = self._column_of_step(i)
@@ -1138,7 +1244,15 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
         perm = self.engine.sort_by_cell(g, el.dev('lon', t.float64), el.dev('lat', t.float64), self._z_for_sampling())
         el.permute(perm)
         self._sorted = True
-        self._env_view = None
+        if getattr(self, '_env_view', None) is not None:
+            # the start-of-step environment follows the elements: sampling it again would see depths the sea-floor interaction
+            # has already lifted (the reference samples once, before it, :2238-2256)
+            self._env_view.permute(perm, self.engine)
+        if getattr(self, '_ssh_now', None) is not None:
+            self._ssh_now = self.engine.permute(perm, self._ssh_now)
+        if getattr(self, '_ssh_prev', None) is not None:
+            self._ssh_prev = self.engine.permute(perm, self._ssh_prev)
+            self.environment_previous = EnvironmentView({'sea_surface_height': self._ssh_prev})
 
     # -- the output buffer (:2100-2135, 2384-2499) -----------------------------------------------------------------------
     # The reference pre-allocates result[var][trajectory, time] for the expected output times, NaN-filled; output steps write

@@ -48,7 +48,7 @@ class OceanDrift(OpenDriftSimulation):
         'sea_surface_wave_stokes_drift_y_velocity': {'fallback': 0, 'skip_if': ['drift:stokes_drift', 'is', False]},
         'ocean_mixed_layer_thickness': {'fallback': 50, 'skip_if': ['drift:vertical_mixing', 'is', False]},
         'sea_floor_depth_below_sea_level': {'fallback': 10000},
-        'sea_surface_height': {'fallback': 0},           # only its fallback is used: a reader for it is refused at run()
+        'sea_surface_height': {'fallback': 0, 'store_previous_if': ['drift:vertical_advection', 'is', True]},
         'land_binary_mask': {'fallback': None},
     }
 
@@ -79,7 +79,9 @@ class OceanDrift(OpenDriftSimulation):
             'drift:water_column_stretching': {'type': 'bool', 'default': False, 'level': CONFIG_LEVEL_ADVANCED,
                                               'description': 'Accepted with the reference\'s default; True is refused at run().'},
             'drift:vertical_advection_correction': {'type': 'bool', 'default': False, 'level': CONFIG_LEVEL_ADVANCED,
-                                                    'description': 'Accepted with the reference\'s default; True is refused at run().'},
+                                                    'description': 'Subtract the vertical motion of the water due to the change in '
+                                                                   'sea surface height from the vertical water velocity '
+                                                                   '(refused in distributed runs).'},
             'drift:use_tabularised_stokes_drift': {'type': 'bool', 'default': False, 'level': CONFIG_LEVEL_BASIC,
                                                    'description': 'Accepted with the reference\'s default; True is refused at run().'},
             'drift:tabularised_stokes_drift_fetch': {'type': 'enum', 'enum': ['5000', '25000', '50000'], 'default': '25000',
@@ -141,9 +143,16 @@ class OceanDrift(OpenDriftSimulation):
     def _overridden_mixing_hooks(self):
         return [h for h in self.MIXING_HOOKS if getattr(type(self), h) is not getattr(OceanDrift, h)]
 
+    def _ssh_reads(self):
+        """Readers of the per-element sea surface height besides the previous-step store: the sea floor (a reader for its depth),
+        vertical mixing, drift:vertical_advection_correction, a bottom_interaction of a subclass (handed -(floor + ssh))."""
+        return (super()._ssh_reads() or bool(self.get_config('drift:vertical_mixing')) or self._vertical_advection_correction()
+                or type(self).bottom_interaction is not OceanDrift.bottom_interaction)
+
     def _buoyancy_inputs(self):
         """(sea floor tensor or None, sea_surface_height, status code for 'deactivate' or 0): the sea-floor part of
-        vertical_buoyancy only acts when a reader provides the depth (interact_with_seafloor, basemodel/__init__.py:752-753)."""
+        vertical_buoyancy only acts when a reader provides the depth (interact_with_seafloor, basemodel/__init__.py:752-753).
+        A per-element sea surface height comes added to the floor (the water column, float32)."""
         if not self.env.priority_list.get('sea_floor_depth_below_sea_level'):
             return None, 0.0, 0
         action = self.get_config('general:seafloor_action')
@@ -151,8 +160,7 @@ class OceanDrift(OpenDriftSimulation):
             return None, 0.0, 0
         if action == 'previous':
             return None, 0.0, 0        # no lift: vertical_buoyancy() moves the elements below the floor back afterwards
-        floor = self._start_of_step_sample('sea_floor_depth_below_sea_level')
-        ssh = float(self.env.constant('sea_surface_height') or self.env.fallback('sea_surface_height') or 0.0)
+        floor, ssh = self._water_column(self._start_of_step_sample('sea_floor_depth_below_sea_level'))
         code = 0
         if action == 'deactivate':
             code = self.status_categories.index('seafloor') if 'seafloor' in self.status_categories else len(self.status_categories)
@@ -182,7 +190,8 @@ class OceanDrift(OpenDriftSimulation):
             self.interact_with_seafloor()          # (:363-366: elements that sank below the floor go back to their previous position)
 
     def vertical_advection(self):
-        """oceandrift.py:315-350: z = min(0, z + moving*w*dt) below (or at) the surface."""
+        """oceandrift.py:315-350: z = min(0, z + moving*w*dt) below (or at) the surface; with drift:vertical_advection_correction
+        w less the vertical motion of the water column due to the change of the sea surface height since the previous step."""
         if self.get_config('drift:vertical_advection') is False:
             return
         env = self.environment
@@ -190,6 +199,15 @@ class OceanDrift(OpenDriftSimulation):
             return
         eng, el, torch = self.engine, self.elements, self.engine.torch
         w = env.dev('upward_sea_water_velocity', eng)
+        if self._vertical_advection_correction() and getattr(self, '_ssh_prev', None) is not None:
+            floor = self._constant_or_none('sea_floor_depth_below_sea_level')
+            if floor is None:
+                floor = env.dev('sea_floor_depth_below_sea_level', eng)
+            z = self._z_for_sampling().clone()
+            eng.vertical_advection_corrected(z, w, self._ssh_tensor(), self._ssh_prev, floor, el.dev('moving', torch.int32),
+                                             self.get_config('drift:vertical_advection_at_surface'), self.time_step.total_seconds())
+            el.set_dev('z', z)
+            return
         z = el.dev('z')
         mv = el.dev('moving').to(torch.float64)
         ok = (z <= 0) if self.get_config('drift:vertical_advection_at_surface') else (z < 0)
@@ -247,6 +265,8 @@ class OceanDrift(OpenDriftSimulation):
         """Run the mixing kernel from start-of-step positions; returns the new float64 depth tensor."""
         eng, el, torch = self.engine, self.elements, self.engine.torch
         g, model, dt_mix, ntimes, floor = self._mixing_inputs()
+        # Zmin = -1.*(sea_floor_depth + sea_surface_height) (:420): the kernel negates the float32 column it is handed
+        floor, _ = self._water_column(floor, tensor=True)
         n = len(el)
         moving = el.dev('moving')
         if moving.dtype != torch.int32:
@@ -314,13 +334,17 @@ class OceanDrift(OpenDriftSimulation):
                 self.surface_stick()
             if 'surface_wave_mixing' in hooks:
                 self.surface_wave_mixing(abs(dt_mix))
-            if action:
-                self._stick_to_bottom(floor, action, code)
+            # 'Let particles stick to bottom' (:557-561): which elements are below -(floor + ssh) is decided before
+            # interact_with_seafloor lifts them; bottom_interaction then gets that Zmin
+            below = False
             if 'bottom_interaction' in hooks:
                 zmin = -(self.environment.sea_floor_depth_below_sea_level + self.environment.sea_surface_height) \
                     if 'sea_surface_height' in self.environment else -self.environment.sea_floor_depth_below_sea_level
-                if (np.asarray(el.z) < zmin).any():
-                    self.bottom_interaction(zmin)
+                below = bool((np.asarray(el.z) < zmin).any())
+            if action:
+                self._stick_to_bottom(floor, action, code)
+            if below:
+                self.bottom_interaction(zmin)
             z = self._z_for_sampling()
         return z
 
@@ -379,6 +403,8 @@ class OceanDrift(OpenDriftSimulation):
             return False        # ensemble blocks: every sample goes through Reader.sample_groups (helper / staged recipes)
         if self.env.has_host_readers():
             return False        # a reader that computes its values on the host (readers/continuous.py): helper / staged recipes
+        if self._vertical_advection_correction():
+            return False        # the corrected vertical advection is a launch of its own after the moves (helper recipe)
         if self.env.priority_list.get('sea_floor_depth_below_sea_level'):
             # A reader for the sea floor: elements below it are lifted at the top of the loop, AFTER the step's environment was
             # sampled (basemodel/__init__.py:2238-2256) -- the first Runge-Kutta stage and w see the depth before the lift, the
