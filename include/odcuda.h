@@ -100,15 +100,23 @@ int od_device_sm_count(od_ctx* ctx);
  * positions are projected before the index arithmetic (Variables.lonlat2xy, readers/basereader/variables.py:129-143; the
  * longitude is modulated first as lon_mode says, :259-280) and, with rotate_vectors, the two components of the group are
  * rotated from the plane's axes to east / north after the interpolation (rotate_vectors, :59-109, :799-837).  Sampled by the
- * general kernels (od_interp, the reader-chain family of step kernels, mixing, Leeway); kind 0 = geographic (+proj=latlong). */
+ * general kernels (od_interp, the reader-chain family of step kernels, mixing, Leeway); kind 0 = geographic (+proj=latlong).
+ * OD_PROJ_OB_TRAN, a rotated pole (+proj=ob_tran +o_proj=longlat +o_lat_p +o_lon_p +lon_0): the axes are rotated longitude /
+ * latitude in degrees.  Its parameters travel in the fields of the other kinds: lon_0 = +lon_0, lat_1 = +o_lat_p,
+ * lat_2 = +o_lon_p, a = +R (the angles do not use it; it must be > 0), k_0 = 1, everything else 0.  As in the reference, the
+ * coverage test takes the rotated x modulated as lon_mode says (covers_positions_xy, variables.py:244-247) and the index
+ * takes np.mod(x, 360) when xmin > 0, the unmodulated x otherwise (basereader/structured.py:213-215); vector pairs are
+ * rotated with a y-axis line of 0.1 degrees. */
 #define OD_PROJ_STERE_SPHERE 1
 #define OD_PROJ_MERC 2
 #define OD_PROJ_LCC 3
 #define OD_PROJ_STERE_ELLPS 4
+#define OD_PROJ_OB_TRAN 5
 typedef struct od_proj_desc {
     int32_t kind;                 /* OD_PROJ_STERE_SPHERE: +proj=stere on a sphere (+R, or +a with +e=0 / +es=0);
                                      OD_PROJ_MERC: +proj=merc; OD_PROJ_LCC: +proj=lcc (+lat_1 [+lat_2]); sphere or ellipsoid (es);
-                                     OD_PROJ_STERE_ELLPS: +proj=stere on an ellipsoid (es > 0), all four aspects */
+                                     OD_PROJ_STERE_ELLPS: +proj=stere on an ellipsoid (es > 0), all four aspects;
+                                     OD_PROJ_OB_TRAN: +proj=ob_tran +o_proj=longlat (fields: see above) */
     int32_t has_lat_ts;           /* +lat_ts given (stere: polar aspects only; merc: the latitude of true scale replaces k_0) */
     double a;                     /* sphere radius / semi-major axis, m */
     double lat_0, lon_0, lat_ts;  /* degrees */

@@ -164,7 +164,7 @@ class PackArgs(C.Structure):
 
 
 OD_PROJ_STERE_SPHERE = 1
-OD_PROJ_MERC, OD_PROJ_LCC, OD_PROJ_STERE_ELLPS = 2, 3, 4
+OD_PROJ_MERC, OD_PROJ_LCC, OD_PROJ_STERE_ELLPS, OD_PROJ_OB_TRAN = 2, 3, 4, 5
 OD_ANALYTIC_DOUBLE_GYRE = 1
 
 # every symbol include/odcuda.h declares: (restype, argtypes)

@@ -452,8 +452,17 @@ OD_HD HorizWP horiz_weights_any(const GroupGeom& g, double lon, double lat, bool
     if (!stere_forward(g.proj, xl, lat, px, py)) return r;
     r.px = px;
     r.py = py;
-    if (!(px >= g.xmin && px <= g.xmax && py >= g.ymin && py <= g.ymax)) return r;
-    double xi = OD_DMUL(div_rn(OD_DSUB(px, g.x0), g.xspan, g.rxspan), g.nxm1);
+    double xc = px;          // x of the coverage test
+    double xx = px;          // x of the index
+    if (g.proj_kind == OD_PROJ_OB_TRAN) {
+        // rotated degrees, which the reference treats as geographic: the coverage test modulates them with the convention of the
+        // reader's TRUE corner longitudes (covers_positions_xy / modulate_longitude, variables.py:244-247, 259-280), the index
+        // takes them mod 360 only when xmin > 0 (basereader/structured.py:213-215) -- the two can disagree, as they do there
+        xc = (g.lon_mode == 0) ? np_mod360(px) : OD_DSUB(np_mod360(OD_DADD(px, 180.0)), 180.0);
+        if (g.xmin > 0.0) xx = np_mod360(px);
+    }
+    if (!(xc >= g.xmin && xc <= g.xmax && py >= g.ymin && py <= g.ymax)) return r;
+    double xi = OD_DMUL(div_rn(OD_DSUB(xx, g.x0), g.xspan, g.rxspan), g.nxm1);
     double yi = OD_DMUL(div_rn(OD_DSUB(py, g.y0), g.yspan, g.ryspan), g.nym1);
     if (!(xi == xi) || !(yi == yi)) return r;
     xi = xi < 0.0 ? 0.0 : (xi > g.nxm1 ? g.nxm1 : xi);

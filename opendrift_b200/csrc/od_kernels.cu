@@ -600,7 +600,8 @@ static GroupGeom make_geom(const Group& g) {
     if (g.desc.proj.kind != 0 && proj_from_desc(&g.desc.proj, &q.proj) == 0) {
         q.proj_kind = g.desc.proj.kind;
         q.rotate = g.desc.rotate_vectors ? 1 : 0;
-        q.rot_delta = 10.0;                        // rotate_vectors: 10 m along the y axis of a projected plane (variables.py:79-82)
+        // rotate_vectors: 10 m along the y axis of a projected plane, 0.1 degrees on a rotated-pole one (variables.py:79-82)
+        q.rot_delta = q.proj_kind == OD_PROJ_OB_TRAN ? kObTranRotDelta : 10.0;
     }
     return q;
 }

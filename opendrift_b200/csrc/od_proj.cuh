@@ -9,6 +9,9 @@
 // 20-14, 20-15, 20-18, 21-15); Mercator (7-1, 7-2 / 7-6 .. 7-9) and Lambert conformal conic with one or two standard
 // parallels (15-1 .. 15-5 / 15-7 .. 15-11, 14-15, 15-9) on a sphere or an ellipsoid, organised like PROJ's merc.cpp / lcc.cpp
 // (msfn, tsfn, phi2); all wrapped in PROJ's generic steps (lam = lon - lon_0 reduced to [-pi, pi], x = a x' + x_0).
+// Rotated pole (+proj=ob_tran +o_proj=longlat, ob_tran.cpp o_forward / o_inverse, Snyder 5-7, 5-8b): the plane is rotated
+// longitude / latitude in DEGREES, as the reference's lonlat2xy / xy2lonlat hand them out (np.degrees of what pyproj returns,
+// variables.py:111-143); a = 1, x_0 = y_0 = 0 so that the generic steps leave those degrees untouched.
 // Geod.inv: only the forward azimuth of a short line is needed; it is obtained by inverting the direct solution
 // (mid-latitude first guess, one correction with the miss of the direct series move) -- the miss shrinks by
 // (s/a)^2 ~ 2e-12 per pass for the 10 m line.
@@ -22,15 +25,16 @@ enum { PROJ_EQUIT = 0, PROJ_OBLIQ = 1, PROJ_N_POLE = 2, PROJ_S_POLE = 3 };
 
 struct ProjStere {               // (the name is historical: kind selects the projection)
     int mode;                    // aspect of the stereographic projection
-    int kind;                    // OD_PROJ_STERE_SPHERE, OD_PROJ_MERC, OD_PROJ_LCC
-    double a, ra, akm1, sinX1, cosX1, phi0, lam0, x0, y0;
+    int kind;                    // OD_PROJ_STERE_SPHERE, OD_PROJ_MERC, OD_PROJ_LCC, OD_PROJ_STERE_ELLPS, OD_PROJ_OB_TRAN
+    double a, ra, akm1, sinX1, cosX1, phi0, lam0, x0, y0;   // (ob_tran: sinX1 / cosX1 of +o_lat_p)
     double e, es;                // eccentricity of the ellipsoid (0: sphere)
     double k0;                   // scale factor (Mercator: from +lat_ts or +k_0; cone: +k_0)
-    double n, c, rho0;           // cone constant, F of Snyder 15-10, radius of the parallel of origin
+    double n, c, rho0;           // cone constant, F of Snyder 15-10, radius of the parallel of origin (ob_tran: n = +o_lon_p, rad)
 };
 
 constexpr double kPi = 3.14159265358979323846;
 constexpr double kHalfPi = 1.57079632679489661923;
+constexpr double kObTranRotDelta = 0.1;          // rotate_vectors' y-axis line on a rotated-pole plane, degrees (variables.py:79-82)
 
 // PROJ adjlon: reduce to [-pi, pi]; values already inside are left untouched
 OD_HD double adjlon(double lam) {
@@ -129,6 +133,16 @@ OD_PROJ_NOINLINE bool proj_forward_other(ProjOther q, double lam, double phi, do
         *oy = py;
         return true;
     }
+    if (q.kind == OD_PROJ_OB_TRAN) {                   // ob_tran.cpp o_forward (its transverse form is the same with o_lat_p = 0)
+        double sl, cl, sp, cp;
+        sincos(lam, &sl, &cl);
+        sincos(phi, &sp, &cp);
+        const double lr = adjlon(atan2(cp * sl, q.sinX1 * cp * cl + q.cosX1 * sp) + q.n);
+        const double pr = asin(fmin(1.0, fmax(-1.0, q.sinX1 * sp - q.cosX1 * cp * cl)));
+        *ox = lr * kRad2Deg;
+        *oy = pr * kRad2Deg;
+        return true;
+    }
     return false;
 }
 
@@ -192,6 +206,14 @@ OD_PROJ_NOINLINE void proj_inverse_other(ProjOther q, double x, double y, double
         const double lm = (xx == 0.0 && yy == 0.0) ? 0.0 : atan2(xx, yy);
         *olam = lm;
         *ophi = ph;
+        return;
+    }
+    if (q.kind == OD_PROJ_OB_TRAN) {                   // ob_tran.cpp o_inverse; x, y are rotated degrees
+        double sl, cl, sp, cp;
+        sincos(x * kDeg - q.n, &sl, &cl);
+        sincos(y * kDeg, &sp, &cp);
+        *ophi = asin(fmin(1.0, fmax(-1.0, q.sinX1 * sp + q.cosX1 * cp * cl)));
+        *olam = atan2(cp * sl, q.sinX1 * cp * cl - q.cosX1 * sp);
         return;
     }
     *olam = 0.0;
@@ -299,7 +321,8 @@ OD_HD double inverse_azimuth_short(double lon1, double lat1, double lon2, double
 // od_proj_desc (include/odcuda.h) -> the per-launch constants; the aspect and scale constant are chosen as PROJ's stere
 // setup does for a sphere.  Returns 0, or 2 unknown projection, 3 bad radius / scale.
 static inline int proj_from_desc(const od_proj_desc* d, ProjStere* Pp) {
-    if (d->kind != OD_PROJ_STERE_SPHERE && d->kind != OD_PROJ_MERC && d->kind != OD_PROJ_LCC && d->kind != OD_PROJ_STERE_ELLPS) return 2;
+    if (d->kind != OD_PROJ_STERE_SPHERE && d->kind != OD_PROJ_MERC && d->kind != OD_PROJ_LCC && d->kind != OD_PROJ_STERE_ELLPS &&
+        d->kind != OD_PROJ_OB_TRAN) return 2;
     if (!(d->a > 0.0) || !(d->k_0 > 0.0)) return 3;
     ProjStere& P = *Pp;
     P.kind = d->kind;
@@ -316,6 +339,17 @@ static inline int proj_from_desc(const od_proj_desc* d, ProjStere* Pp) {
     P.n = P.c = P.rho0 = 0.0;
     P.mode = 0;
     P.akm1 = P.sinX1 = P.cosX1 = 0.0;
+    if (d->kind == OD_PROJ_OB_TRAN) {                  // ob_tran.cpp setup, new-pole form: lat_1 = +o_lat_p, lat_2 = +o_lon_p (degrees)
+        if (!(fabs(d->lat_1) <= 90.0) || !(fabs(d->lat_2) <= 360.0)) return 3;
+        P.a = P.ra = 1.0;                              // the plane is rotated degrees: no radius, no false origin
+        P.x0 = P.y0 = 0.0;
+        P.es = P.e = 0.0;
+        P.k0 = 1.0;
+        P.sinX1 = sin(d->lat_1 * kDeg);
+        P.cosX1 = cos(d->lat_1 * kDeg);
+        P.n = d->lat_2 * kDeg;
+        return 0;
+    }
     if (d->kind == OD_PROJ_MERC) {                     // merc.cpp: +lat_ts replaces +k_0
         if (d->has_lat_ts) {
             const double phits = fabs(d->lat_ts * kDeg);
@@ -377,8 +411,11 @@ static inline int proj_from_desc(const od_proj_desc* d, ProjStere* Pp) {
 }
 
 // rotate_vectors (variables.py:59-109): angle (radians) by which components along the plane's x / y axes at (px, py) are
-// rotated to become east / north components
+// rotated to become east / north components.  delta is the length of the line along the y axis: 10 m on a projected plane;
+// 0.1 (degrees) on a rotated-pole plane, which pyproj calls geographic (:79-82) -- the kind decides that one, so that it holds
+// whatever geometry the caller built.
 OD_HD double rotation_to_geographic(const ProjStere& P, double px, double py, double delta) {
+    if (P.kind == OD_PROJ_OB_TRAN) delta = kObTranRotDelta;
     double lon1, lat1, lon2, lat2;
     stere_inverse(P, px, py, lon1, lat1);
     stere_inverse(P, px, py + delta, lon2, lat2);

@@ -105,12 +105,16 @@ class StructuredReader:
 
     def __init__(self):
         p = str(getattr(self, 'proj4', '+proj=latlong'))
-        self.proj = None               # a projected plane (+proj=stere on a sphere, +proj=merc, +proj=lcc): x / y axes and xmin .. ymax are metres in it
-        if not any(k in p for k in ('latlong', 'longlat', 'lonlat', 'latlon')):      # PROJ's aliases of the geographic CRS
-            from .projection import make_projection
+        # a projected plane (+proj=stere, +proj=merc, +proj=lcc): x / y axes and xmin .. ymax are metres in it; a rotated pole
+        # (+proj=ob_tran +o_proj=longlat): they are rotated longitude / latitude in degrees
+        self.proj = None
+        from .projection import RotatedPole, is_geographic, make_projection
+        if not is_geographic(p):
             self.proj = make_projection(p)             # raises for what the device code does not project
             if self.subblocks:
                 raise NotImplementedError('sub-block readers on a projected plane are not on the GPU path')
+            if isinstance(self.proj, RotatedPole):
+                self._check_rotated_grid()
             # modulate_longitude (variables.py:259-280): the longitude convention follows the corner longitudes
             exlons, _ = self.proj(np.array([self.xmin, self.xmin, self.xmax, self.xmax], dtype=np.float64),
                                   np.array([self.ymin, self.ymax, self.ymax, self.ymin], dtype=np.float64), inverse=True)
@@ -130,6 +134,16 @@ class StructuredReader:
         self._window = None        # ... and the extent (xmin, xmax, ymin, ymax) of the block that came back
         self._block_caches = []
         self.windows_set = 0
+
+    def _check_rotated_grid(self):
+        """A rotated-pole grid that the reference would treat as global east-west (variables.py:289-301: it tests the rotated
+        axis as if it were longitude), or whose y-axis line of rotate_vectors (0.1 degrees north in the rotated plane) could cross
+        the rotated pole, is refused."""
+        dx = getattr(self, 'delta_x', None) or 0
+        if (self.xmin - 2 * dx <= 0 and self.xmax + 2 * dx >= 360) or (self.xmin - 2 * dx <= -180 and self.xmax + 2 * dx >= 180):
+            raise NotImplementedError('a rotated-pole grid spanning 360 degrees of rotated longitude is not on the GPU path')
+        if self.ymax + 0.1 >= 90 or self.ymin - 0.1 <= -90:
+            raise NotImplementedError('a rotated-pole grid within 0.1 degrees of the rotated pole is not on the GPU path')
 
     # -- coverage (variables.py:229-257, 391-400) ------------------------------------------------
     def covers_time(self, time):
@@ -172,7 +186,10 @@ class StructuredReader:
         if self.global_coverage():             # north-south only (variables.py:239-242)
             ind = np.where((y >= self.ymin) & (y <= self.ymax))[0]
         else:
-            ind = np.where((x >= self.xmin) & (x <= self.xmax) & (y >= self.ymin) & (y <= self.ymax))[0]
+            # a rotated pole is geographic to pyproj: its rotated x is tested after modulate_longitude, whose convention comes
+            # from the TRUE corner longitudes (variables.py:244-247, 259-280) -- an element can fall outside a grid it lies on
+            xx = self.modulate_longitude(x) if self._rotated() else x
+            ind = np.where((xx >= self.xmin) & (xx <= self.xmax) & (y >= self.ymin) & (y <= self.ymax))[0]
         return ind, x[ind], y[ind]
 
     def check_arguments(self, variables, time, x, y, z):
@@ -194,7 +211,11 @@ class StructuredReader:
         dx = getattr(self, 'delta_x', None)
         if dx is None:
             return None
-        return dx if self.proj is not None else dx * 111000   # degrees -> metres for geographic readers
+        return dx if self.proj is not None and not self._rotated() else dx * 111000   # degrees -> metres (also rotated degrees)
+
+    def _rotated(self):
+        from .projection import RotatedPole
+        return isinstance(self.proj, RotatedPole)
 
     def set_buffer_size(self, max_speed, time_coverage=None):
         """Cells added around the requested positions so that the block still covers the elements at the end of the

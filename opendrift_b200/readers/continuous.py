@@ -22,7 +22,8 @@ class ContinuousReader:
 
     def __init__(self):
         p = str(getattr(self, 'proj4', '+proj=latlong'))
-        if not any(k in p for k in ('latlong', 'longlat', 'lonlat', 'latlon')):
+        from .projection import is_geographic
+        if not is_geographic(p):                   # (a rotated pole, +o_proj=longlat, is not geographic)
             raise NotImplementedError('ContinuousReader subclasses on a projected plane are not on the GPU path (got %r); the '
                                       'projected analytical reader that is: readers/reader_double_gyre.py' % p)
         self.zmin, self.zmax = -np.inf, np.inf

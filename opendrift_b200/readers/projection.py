@@ -6,7 +6,7 @@ proj4 string into the library's od_proj_desc and mirrors the same closed forms i
 
 Supported: '+proj=stere' on a sphere ('+R=...' or '+a=... +e=0') or an ellipsoid, all four aspects (Snyder 1987, ch. 21);
 '+proj=merc' and '+proj=lcc' (one or two standard parallels) on a sphere or an ellipsoid (Snyder ch. 7 and 15; PROJ's merc.cpp /
-lcc.cpp).
+lcc.cpp); the rotated pole '+proj=ob_tran +o_proj=longlat +o_lat_p=.. [+o_lon_p=..] +lon_0=..', whose plane is rotated degrees.
 """
 import re
 
@@ -32,6 +32,9 @@ def parse_proj4(s):
 
 
 def is_geographic(proj4):
+    """A plain longitude / latitude grid.  A rotated pole (+proj=ob_tran +o_proj=longlat) is not one: its axes are rotated."""
+    if is_rotated_pole(proj4):
+        return False
     return any(k in str(proj4) for k in ('latlong', 'longlat', 'lonlat', 'latlon'))
 
 
@@ -397,8 +400,71 @@ def _is_sphere(proj4):
     return es == 0.0
 
 
+def is_rotated_pole(proj4):
+    return parse_proj4(proj4).get('proj') == 'ob_tran'
+
+
+class RotatedPole:
+    """+proj=ob_tran +o_proj=longlat in its new-pole form (+o_lat_p, +o_lon_p, +lon_0; PROJ's ob_tran.cpp o_forward / o_inverse,
+    Snyder 1987 eqs. 5-7 and 5-8b): the reader's plane is rotated longitude / latitude in DEGREES -- what the reference's lonlat2xy
+    and xy2lonlat hand out around pyproj's radians (variables.py:111-143).  The rotation does not depend on the radius."""
+    kind = _lib.OD_PROJ_OB_TRAN
+    _REFUSED = ('to_meter', 'o_alpha', 'o_lon_c', 'o_lat_c', 'o_lon_1', 'o_lat_1', 'o_lon_2', 'o_lat_2', 'o_lon_b', 'o_lat_b')
+
+    def __init__(self, proj4):
+        p = parse_proj4(proj4)
+        if p.get('proj') != 'ob_tran':
+            raise NotImplementedError(proj4)
+        if p.get('o_proj') not in ('longlat', 'lonlat', 'latlong'):
+            raise NotImplementedError('+proj=ob_tran on the GPU path: +o_proj=longlat only; got %s' % proj4)
+        bad = [k for k in self._REFUSED if k in p]
+        if bad or 'o_lat_p' not in p:
+            raise NotImplementedError('+proj=ob_tran on the GPU path: the +o_lat_p [+o_lon_p] form without +to_meter; got %s' % proj4)
+        if any(float(p.get(k, 0.0)) != 0.0 for k in ('x_0', 'y_0')) or float(p.get('k_0', p.get('k', 1.0))) != 1.0:
+            raise NotImplementedError('+proj=ob_tran with a false origin or a scale factor: %s' % proj4)
+        self.proj4, self.p = str(proj4), p
+        self.a = float(p['R']) if 'R' in p else float(p.get('a', 6378137.0))
+        self.lon_0 = float(p.get('lon_0', 0.0))
+        self.o_lat_p = float(p['o_lat_p'])
+        self.o_lon_p = float(p.get('o_lon_p', 0.0))
+        if not (abs(self.o_lat_p) <= 90.0):
+            raise ValueError('+o_lat_p must lie in [-90, 90]: %s' % proj4)
+        self.lam0, self.lamp = self.lon_0 * _DEG, self.o_lon_p * _DEG
+        self.sphip, self.cphip = np.sin(self.o_lat_p * _DEG), np.cos(self.o_lat_p * _DEG)
+
+    def desc(self):
+        d = _lib.ProjDesc()
+        d.kind = self.kind
+        d.a, d.lon_0, d.k_0 = self.a, self.lon_0, 1.0
+        d.lat_1, d.lat_2 = self.o_lat_p, self.o_lon_p
+        return d
+
+    _adjlon = staticmethod(SphericalStereographic._adjlon)
+
+    def __call__(self, a, b, inverse=False):
+        scalar = np.isscalar(a)
+        a = np.atleast_1d(np.asarray(a, dtype=np.float64))
+        b = np.atleast_1d(np.asarray(b, dtype=np.float64))
+        with np.errstate(all='ignore'):
+            if inverse:
+                lam, phi = np.radians(a) - self.lamp, np.radians(b)
+                sl, cl, sp, cp = np.sin(lam), np.cos(lam), np.sin(phi), np.cos(phi)
+                ra = np.degrees(self._adjlon(np.arctan2(cp * sl, self.sphip * cp * cl - self.cphip * sp) + self.lam0))
+                rb = np.degrees(np.arcsin(np.clip(self.sphip * sp + self.cphip * cp * cl, -1, 1)))
+            else:
+                lam, phi = self._adjlon(a * _DEG - self.lam0), b * _DEG
+                sl, cl, sp, cp = np.sin(lam), np.cos(lam), np.sin(phi), np.cos(phi)
+                ra = np.degrees(self._adjlon(np.arctan2(cp * sl, self.sphip * cp * cl + self.cphip * sp) + self.lamp))
+                rb = np.degrees(np.arcsin(np.clip(self.sphip * sp - self.cphip * cp * cl, -1, 1)))
+        if scalar:
+            return float(ra[0]), float(rb[0])
+        return ra, rb
+
+
 def make_projection(proj4):
     """The projection object of a reader's proj4 string (None for a geographic reader)."""
+    if is_rotated_pole(proj4):                 # (before the geographic test: its +o_proj=longlat names a geographic CRS)
+        return RotatedPole(proj4)
     if is_geographic(proj4):
         return None
     name = parse_proj4(proj4).get('proj')
