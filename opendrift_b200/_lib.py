@@ -7,7 +7,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get('ODCUDA_LIB') or os.path.join(_HERE, 'libodcuda.so')   # ODCUDA_LIB: tuning builds only
+LIB_PATH = os.environ.get('ODCUDA_LIB') or os.path.join(_HERE, 'libodcuda.so')   # ODCUDA_LIB: another build, to compare two builds
 
 OD_EULER, OD_RK2, OD_RK4 = 0, 1, 2
 OD_T_LERP, OD_T_FIRST, OD_T_SECOND, OD_T_MISSING = 0, 1, 2, 3

@@ -75,21 +75,21 @@ struct od_ctx {
     int32_t* d_bins = nullptr;
     int64_t keys_cap = 0, bins_cap = 0;
     int32_t* d_tilesums = nullptr;      // tile totals of the two-level scan
-    int tiles_cap = 0;
+    int64_t tiles_cap = 0;
     unsigned* d_red = nullptr;          // reduction scratch
     unsigned long long* d_bbox = nullptr;   // od_bbox's four extrema
     unsigned* d_cnt = nullptr;          // counters of the housekeeping kernels
     float* d_fill = nullptr;            // scratch slab of the NaN fill
     unsigned* d_fillcnt = nullptr;      // per-pass missing-cell counters
-    int coop_fill_blocks = -1;          // co-resident grid of fill_nan_coop_kernel (0: no cooperative launch)
+    int coop_fill_blocks = -1;          // co-resident grid of fill_nan_coop_kernel (0: the device cannot launch it)
     int64_t fill_cap = 0;
     int tile = 0;                       // OD_OPT_TILE: stage field boxes in shared memory with TMA
     int spec = 1;                       // OD_OPT_SPEC: launches that qualify take the specialised step kernel (od_spec.cuh)
-    // host-array pipeline (od_advect_current_host): three streams, three staging buffers
+    // host-array pipeline (od_advect_current_host): three streams, three staging buffers back to back in hbuf
     cudaStream_t hstream[3] = {nullptr, nullptr, nullptr};
     cudaEvent_t hready = nullptr;
-    char* hbuf[3] = {nullptr, nullptr, nullptr};
-    int64_t hbuf_cap = 0;               // particles per staging buffer
+    char* hbuf = nullptr;
+    int64_t hbuf_cap = 0;               // particles per staging buffer (24 bytes each)
 };
 
 static inline int fail(od_ctx* c, int code, const char* what, cudaError_t e = cudaSuccess) {

@@ -71,10 +71,9 @@ extern "C" void od_destroy(od_ctx* ctx) {
     if (ctx->d_fill) cudaFree(ctx->d_fill);
     if (ctx->d_fillcnt) cudaFree(ctx->d_fillcnt);
     if (ctx->d_tilesums) cudaFree(ctx->d_tilesums);
-    for (int k = 0; k < 3; ++k) {
-        if (ctx->hbuf[k]) cudaFree(ctx->hbuf[k]);
+    if (ctx->hbuf) cudaFree(ctx->hbuf);
+    for (int k = 0; k < 3; ++k)
         if (ctx->hstream[k]) cudaStreamDestroy(ctx->hstream[k]);
-    }
     if (ctx->hready) cudaEventDestroy(ctx->hready);
     delete ctx;
 }
@@ -191,12 +190,19 @@ extern "C" int od_group_upload(od_ctx* ctx, int group, int slot, int comp, const
     return OD_OK;
 }
 
+// Grow-only scratch: *p holds at least `need` elements of `elem` bytes afterwards; a buffer that is large enough is kept.
+// A failed allocation leaves *p null and *cap 0, so that the next call allocates again.
+static int grow(od_ctx* ctx, void** p, int64_t* cap, int64_t need, size_t elem) {
+    if (*cap >= need) return OD_OK;
+    if (*p) cudaFree(*p);
+    *p = nullptr;
+    *cap = 0;
+    CK(cudaMalloc(p, (size_t)need * elem));
+    *cap = need;
+    return OD_OK;
+}
+
 #define OD_FILL_MAX_IT 16
-__global__ void dilate_nan_kernel(const float* __restrict__ src, float* __restrict__ dst, int nx, int ny, int64_t cells,
-                                  const unsigned* __restrict__ missing_before, unsigned* __restrict__ missing_after);
-__global__ void dilate_commit_kernel(const float* __restrict__ src, float* __restrict__ dst, int64_t cells,
-                                     const unsigned* __restrict__ missing_before);
-__global__ void count_nonfinite_kernel(const float* __restrict__ a, int64_t cells, unsigned* __restrict__ counters);
 __global__ void fill_nan_coop_kernel(float* a, float* tmp, int nx, int ny, int64_t cells, int max_iterations, unsigned* cnt);
 
 extern "C" int od_group_fill_nan(od_ctx* ctx, int group, int slot, int comp, int max_iterations, int64_t* h_remaining) {
@@ -205,22 +211,7 @@ extern "C" int od_group_fill_nan(od_ctx* ctx, int group, int slot, int comp, int
     if (max_iterations < 0 || max_iterations > OD_FILL_MAX_IT) return fail(ctx, OD_ERR_ARG, "od_group_fill_nan: bad iteration count");
     Group& g = ctx->groups[group];
     CK(cudaSetDevice(ctx->device));
-    const int64_t cells = (int64_t)g.cells();
-    float* a = g.slots[(size_t)slot * g.desc.ncomp + comp];
-    if (!ctx->d_fillcnt) CK(cudaMalloc(&ctx->d_fillcnt, (OD_FILL_MAX_IT + 2) * sizeof(unsigned)));
-    if (ctx->fill_cap < cells) {                     // grow-only scratch slab (allocated once per context)
-        if (ctx->d_fill) cudaFree(ctx->d_fill);
-        ctx->d_fill = nullptr;
-        CK(cudaMalloc(&ctx->d_fill, cells * sizeof(float)));
-        ctx->fill_cap = cells;
-    }
-    // Everything below is enqueued without a host round trip: counters[it] = cells still missing before pass `it`;
-    // a pass whose counter is zero returns at once, so a slab without holes costs one read pass.
-    unsigned* cnt = ctx->d_fillcnt;
-    CK(cudaMemsetAsync(cnt, 0, (OD_FILL_MAX_IT + 2) * sizeof(unsigned), ctx->stream));
-    int blocks = (int)((cells + 255) / 256);
-    const int capped = blocks > ctx->sm_count * 16 ? ctx->sm_count * 16 : blocks;
-    if (ctx->coop_fill_blocks < 0) {                 // once: can the whole grid be co-resident (cooperative launch)?
+    if (ctx->coop_fill_blocks < 0) {                 // once: how many blocks of the fill can be co-resident (cooperative launch)?
         int per_sm = 0, coop = 0;
         cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, ctx->device);
         if (coop && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, fill_nan_coop_kernel, 256, 0) == cudaSuccess && per_sm > 0)
@@ -233,25 +224,24 @@ extern "C" int od_group_fill_nan(od_ctx* ctx, int group, int slot, int comp, int
             ctx->coop_fill_blocks = 0;
         cudaGetLastError();
     }
-    if (ctx->coop_fill_blocks > 0) {
-        int gridc = blocks < ctx->coop_fill_blocks ? blocks : ctx->coop_fill_blocks;
-        float* tmp = ctx->d_fill;
-        int nx = g.desc.nx, ny = g.desc.ny;
-        int64_t ncells = cells;
-        int mit = max_iterations;
-        void* args[] = {&a, &tmp, &nx, &ny, &ncells, &mit, &cnt};
-        CK(cudaLaunchCooperativeKernel((const void*)fill_nan_coop_kernel, dim3(gridc), dim3(256), args, 0, ctx->stream));
-        ctx->launches++;
-    } else {
-        count_nonfinite_kernel<<<capped, 256, 0, ctx->stream>>>(a, cells, cnt);
-        ctx->launches++;
-        for (int it = 0; it < max_iterations; ++it) {
-            dilate_nan_kernel<<<capped, 256, 0, ctx->stream>>>(a, ctx->d_fill, g.desc.nx, g.desc.ny, cells, cnt + it, cnt + it + 1);
-            dilate_commit_kernel<<<capped, 256, 0, ctx->stream>>>(ctx->d_fill, a, cells, cnt + it);
-            ctx->launches += 2;
-        }
-    }
-    CK(cudaGetLastError());
+    if (ctx->coop_fill_blocks == 0)
+        return fail(ctx, OD_ERR_CUDA, "od_group_fill_nan: the device cannot launch fill_nan_coop_kernel cooperatively");
+    float* a = g.slots[(size_t)slot * g.desc.ncomp + comp];
+    int64_t cells = (int64_t)g.cells();
+    if (!ctx->d_fillcnt) CK(cudaMalloc(&ctx->d_fillcnt, (OD_FILL_MAX_IT + 2) * sizeof(unsigned)));
+    rc = grow(ctx, (void**)&ctx->d_fill, &ctx->fill_cap, cells, sizeof(float));
+    if (rc) return rc;
+    // Everything below is enqueued without a host round trip: cnt[it] = cells still missing before pass `it`;
+    // the passes stop once it is zero, so a slab without holes costs one read pass.
+    unsigned* cnt = ctx->d_fillcnt;
+    CK(cudaMemsetAsync(cnt, 0, (OD_FILL_MAX_IT + 2) * sizeof(unsigned), ctx->stream));
+    const int blocks = (int)((cells + 255) / 256);
+    const int gridc = blocks < ctx->coop_fill_blocks ? blocks : ctx->coop_fill_blocks;
+    float* tmp = ctx->d_fill;
+    int nx = g.desc.nx, ny = g.desc.ny;
+    void* args[] = {&a, &tmp, &nx, &ny, &cells, &max_iterations, &cnt};
+    CK(cudaLaunchCooperativeKernel((const void*)fill_nan_coop_kernel, dim3(gridc), dim3(256), args, 0, ctx->stream));
+    ctx->launches++;
     g.version[slot] = ++ctx->tick;
     if (h_remaining) {                               // optional: the caller asks how many cells stayed missing (synchronises)
         unsigned res = 0;
@@ -366,45 +356,7 @@ extern "C" int od_group_set_fallback(od_ctx* ctx, int group, float fallback0, fl
 // as some particle still interpolates to NaN, at most 10 times (:121-139); the mutation persists in the cached
 // block.  A filled cell never changes again and finite cells are never touched, so filling a block 10 times
 // when it is uploaded gives every particle inside the block the value the reference's lazy loop would give.
-__global__ void __launch_bounds__(256) dilate_nan_kernel(const float* __restrict__ src, float* __restrict__ dst, int nx, int ny,
-                                                         int64_t cells, const unsigned* __restrict__ missing_before,
-                                                         unsigned* __restrict__ missing_after) {
-    if (*missing_before == 0) return;                // nothing left to fill: this pass is a no-op
-    const int64_t layer = (int64_t)nx * ny;
-    unsigned still = 0;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (int64_t)gridDim.x * blockDim.x) {
-        const float v = src[i];
-        if (fabsf(v) <= 3.4028234663852886e38f) {    // finite: unchanged
-            dst[i] = v;
-            continue;
-        }
-        const int64_t base = (i / layer) * layer;
-        const int r = (int)((i - base) / nx), c = (int)((i - base) % nx);
-        float best = -INFINITY;
-        bool found = false;
-        for (int dr = -1; dr <= 1; ++dr) {
-            const int rr = min(max(r + dr, 0), ny - 1);
-            for (int dc = -1; dc <= 1; ++dc) {
-                const int cc = min(max(c + dc, 0), nx - 1);
-                const float w = src[base + (int64_t)rr * nx + cc];
-                if (fabsf(w) <= 3.4028234663852886e38f) {
-                    best = fmaxf(best, w);
-                    found = true;
-                }
-            }
-        }
-        dst[i] = found ? best : NAN;
-        still += found ? 0u : 1u;
-    }
-    if (still) atomicAdd(missing_after, still);
-}
-
-__global__ void __launch_bounds__(256) dilate_commit_kernel(const float* __restrict__ src, float* __restrict__ dst, int64_t cells,
-                                                            const unsigned* __restrict__ missing_before) {
-    if (*missing_before == 0) return;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (int64_t)gridDim.x * blockDim.x) dst[i] = src[i];
-}
-
+//
 // All passes of the fill in one cooperative launch: count, then (dilate, commit) until nothing is missing or
 // max_iterations passes ran.  A slab without holes costs one read pass and one grid barrier.
 __global__ void __launch_bounds__(256) fill_nan_coop_kernel(float* a, float* tmp, int nx, int ny,
@@ -449,14 +401,6 @@ __global__ void __launch_bounds__(256) fill_nan_coop_kernel(float* a, float* tmp
         for (int64_t i = first; i < cells; i += stride) a[i] = tmp[i];
         grid.sync();
     }
-}
-
-__global__ void __launch_bounds__(256) count_nonfinite_kernel(const float* __restrict__ a, int64_t cells, unsigned* __restrict__ counters) {
-    unsigned c = 0;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (int64_t)gridDim.x * blockDim.x)
-        c += !(fabsf(a[i]) <= 3.4028234663852886e38f);
-    for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-    if ((threadIdx.x & 31) == 0 && c) atomicAdd(&counters[0], c);
 }
 
 // interleave two time slabs (and two components) into pair texels
@@ -659,13 +603,20 @@ __global__ void __launch_bounds__(OD_BLOCK) interp_kernel(const InterpParams p) 
     }
 }
 
+// counters[b] += the lanes of this warp whose flags have bit b set, for b < K: one atomic per warp and non-zero count.
+// Every lane of the warp calls it.
+template <int K>
+__device__ __forceinline__ void tally_flags(unsigned* counters, int flags) {
+#pragma unroll
+    for (int b = 0; b < K; ++b) {
+        const unsigned m = __ballot_sync(0xffffffffu, (flags >> b) & 1);
+        if (m && (threadIdx.x & 31) == 0) atomicAdd(counters + b, (unsigned)__popc(m));
+    }
+}
+
 __global__ void __launch_bounds__(256) coast_kernel(const CoastParams p) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int f = i < p.n ? coast_one(p, i) : 0;
-    for (int b = 0; b < 4; ++b) {
-        const unsigned m = __ballot_sync(0xffffffffu, (f >> b) & 1);
-        if (m && (threadIdx.x & 31) == 0) atomicAdd(p.counters + b, (unsigned)__popc(m));
-    }
+    tally_flags<4>(p.counters, i < p.n ? coast_one(p, i) : 0);
 }
 
 __global__ void __launch_bounds__(256) store_previous_kernel(int64_t n, const double* __restrict__ lon, const double* __restrict__ lat,
@@ -892,12 +843,8 @@ static int scan_exclusive(od_ctx* ctx, int32_t* bins, int nbins) {
         return OD_OK;
     }
     const int ntiles = (nbins + OD_SCAN_TILE - 1) / OD_SCAN_TILE;
-    if (ctx->tiles_cap < ntiles) {
-        if (ctx->d_tilesums) cudaFree(ctx->d_tilesums);
-        ctx->d_tilesums = nullptr;
-        CK(cudaMalloc(&ctx->d_tilesums, (size_t)ntiles * sizeof(int32_t)));
-        ctx->tiles_cap = ntiles;
-    }
+    const int rc = grow(ctx, (void**)&ctx->d_tilesums, &ctx->tiles_cap, ntiles, sizeof(int32_t));
+    if (rc) return rc;
     scan_tiles_kernel<<<ntiles, 1024, 0, ctx->stream>>>(bins, nbins, ctx->d_tilesums);
     scan_bins_kernel<<<1, 1024, 0, ctx->stream>>>(ctx->d_tilesums, ntiles);
     add_tile_offsets_kernel<<<ntiles, 1024, 0, ctx->stream>>>(bins, nbins, ctx->d_tilesums);
@@ -968,8 +915,6 @@ __global__ void __launch_bounds__(OD_BLOCK) permute_kernel(int64_t n, const int3
 //           the element's columns are copied into its record
 // The receiving side scatters the records back into SoA columns (unpack_records_kernel).
 #define OD_PACK_BLOCK 256
-#define OD_PACK_MAX_COLS 16
-#define OD_PACK_MAX_WORLD 64
 
 struct PackParams {
     int64_t n;
@@ -987,6 +932,14 @@ __device__ __forceinline__ int strip_of(const PackParams& p, double x) {
     for (int k = 1; k < p.world; ++k) o += (x >= p.bounds[k]) ? 1 : 0;
     if (!(x == x)) o = p.world - 1;
     return o;
+}
+
+// one field of a record, column -> record or back: b bytes at byte offset off of records of rec_bytes; a 4- or 8-byte
+// field that every record keeps aligned moves as one word
+__device__ __forceinline__ void copy_field(unsigned char* dst, const unsigned char* src, int b, int off, int rec_bytes) {
+    if (b == 8 && ((off | rec_bytes) & 7) == 0) *reinterpret_cast<uint64_t*>(dst) = *reinterpret_cast<const uint64_t*>(src);
+    else if (b == 4 && ((off | rec_bytes) & 3) == 0) *reinterpret_cast<uint32_t*>(dst) = *reinterpret_cast<const uint32_t*>(src);
+    else for (int k = 0; k < b; ++k) dst[k] = src[k];
 }
 
 __global__ void __launch_bounds__(OD_PACK_BLOCK) owner_count_kernel(const __grid_constant__ PackParams p, int32_t* __restrict__ table) {
@@ -1018,14 +971,8 @@ __global__ void __launch_bounds__(OD_PACK_BLOCK) owner_pack_kernel(const __grid_
     const int64_t row = (int64_t)table[(int64_t)owner * p.nblocks + blockIdx.x] + before + rank_in_warp;
     if (perm) perm[row] = (int32_t)i;
     unsigned char* rec = records + row * p.rec_bytes;
-    for (int c = 0; c < p.ncols; ++c) {
-        const int b = p.col_bytes[c];
-        const unsigned char* src = p.cols[c] + i * b;
-        unsigned char* dst = rec + p.col_off[c];
-        if (b == 8 && ((p.col_off[c] | p.rec_bytes) & 7) == 0) *reinterpret_cast<uint64_t*>(dst) = *reinterpret_cast<const uint64_t*>(src);
-        else if (b == 4 && ((p.col_off[c] | p.rec_bytes) & 3) == 0) *reinterpret_cast<uint32_t*>(dst) = *reinterpret_cast<const uint32_t*>(src);
-        else for (int k = 0; k < b; ++k) dst[k] = src[k];
-    }
+    for (int c = 0; c < p.ncols; ++c)
+        copy_field(rec + p.col_off[c], p.cols[c] + i * p.col_bytes[c], p.col_bytes[c], p.col_off[c], p.rec_bytes);
 }
 
 struct UnpackParams {
@@ -1040,14 +987,8 @@ __global__ void __launch_bounds__(OD_PACK_BLOCK) unpack_records_kernel(const __g
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= p.n) return;
     const unsigned char* rec = records + i * p.rec_bytes;
-    for (int c = 0; c < p.ncols; ++c) {
-        const int b = p.col_bytes[c];
-        const unsigned char* src = rec + p.col_off[c];
-        unsigned char* dst = p.cols[c] + i * b;
-        if (b == 8 && ((p.col_off[c] | p.rec_bytes) & 7) == 0) *reinterpret_cast<uint64_t*>(dst) = *reinterpret_cast<const uint64_t*>(src);
-        else if (b == 4 && ((p.col_off[c] | p.rec_bytes) & 3) == 0) *reinterpret_cast<uint32_t*>(dst) = *reinterpret_cast<const uint32_t*>(src);
-        else for (int k = 0; k < b; ++k) dst[k] = src[k];
-    }
+    for (int c = 0; c < p.ncols; ++c)
+        copy_field(p.cols[c] + i * p.col_bytes[c], rec + p.col_off[c], p.col_bytes[c], p.col_off[c], p.rec_bytes);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1184,7 +1125,11 @@ static const PairEntry* find_tmap(const Group& g, const float* tex) {
 }
 
 template <int EXTRAS>
-static int launch_step_mode(od_ctx* ctx, int mode, int scheme, bool f64, const StepParams& p);
+static int launch_step_mode(od_ctx* ctx, int mode, int scheme, bool f64, const StepParams& p) {
+    if (mode == OD_MATH_FAST) return launch_step<EXTRAS, FastMath>(ctx, scheme, f64, p);
+    if (mode == OD_MATH_SERIES) return launch_step<EXTRAS, SeriesMath>(ctx, scheme, f64, p);
+    return launch_step<EXTRAS, ExactMath>(ctx, scheme, f64, p);
+}
 
 extern "C" int od_advect_current(od_ctx* ctx, const od_advect_args* a) {
     if (!ctx || !a) return fail(ctx, OD_ERR_ARG, "od_advect_current: null argument");
@@ -1211,8 +1156,6 @@ extern "C" int od_advect_current(od_ctx* ctx, const od_advect_args* a) {
 // fills and drains faster.  Pinned host memory is needed for the copies to overlap.  Returns when the results are in
 // h_out_lon / h_out_lat.
 static int fill_step(od_ctx* ctx, const od_step_args* a, StepParams* pp);
-template <int EXTRAS>
-static int launch_step_mode(od_ctx* ctx, int mode, int scheme, bool f64, const StepParams& p);
 
 static int host_pipeline(od_ctx* ctx, const od_advect_args* a, const od_step_args* step, const od_host_io* io) {
     const int64_t n = a->n;
@@ -1255,15 +1198,8 @@ static int host_pipeline(od_ctx* ctx, const od_advect_args* a, const od_step_arg
     const double unit = chunks > 2 ? (double)n / (chunks - 1) : (double)n / chunks;
     const int64_t cap = (int64_t)unit + 2;
     const size_t zsz = a->z_f64 ? 8 : 4;
-    if (ctx->hbuf_cap < cap) {
-        for (int k = 0; k < 3; ++k) {
-            if (ctx->hbuf[k]) cudaFree(ctx->hbuf[k]);
-            ctx->hbuf[k] = nullptr;
-        }
-        ctx->hbuf_cap = 0;
-        for (int k = 0; k < 3; ++k) CK(cudaMalloc(&ctx->hbuf[k], (size_t)cap * 24));      // lon, lat (float64), z (<= 8 B)
-        ctx->hbuf_cap = cap;
-    }
+    rc = grow(ctx, (void**)&ctx->hbuf, &ctx->hbuf_cap, cap, 3 * 24);        // three buffers of lon, lat (float64), z (<= 8 B)
+    if (rc) return rc;
     CK(cudaEventRecord(ctx->hready, ctx->stream));
     static const bool trace = getenv("OD_HOST_TRACE") != nullptr;       // debugging aid: per-chunk timeline on stderr
     std::vector<cudaEvent_t> tev;
@@ -1293,7 +1229,7 @@ static int host_pipeline(od_ctx* ctx, const od_advect_args* a, const od_step_arg
         if (m <= 0) continue;
         const int k = c % 3;
         cudaStream_t st = ctx->hstream[k];
-        double* d_lon = (double*)ctx->hbuf[k];
+        double* d_lon = (double*)(ctx->hbuf + k * ctx->hbuf_cap * 24);
         double* d_lat = d_lon + ctx->hbuf_cap;
         char* d_z = (char*)(d_lat + ctx->hbuf_cap);
         if (c < 3) CK(cudaStreamWaitEvent(st, ctx->hready, 0));
@@ -1398,17 +1334,6 @@ static int fill_step(od_ctx* ctx, const od_step_args* a, StepParams* pp) {
     return OD_OK;
 }
 
-template <int EXTRAS>
-static int launch_step_mode(od_ctx* ctx, int mode, int scheme, bool f64, const StepParams& p) {
-    if (mode == OD_MATH_FAST) return launch_step<EXTRAS, FastMath>(ctx, scheme, f64, p);
-    if (mode == OD_MATH_SERIES) return launch_step<EXTRAS, SeriesMath>(ctx, scheme, f64, p);
-#ifdef OD_SLIM
-    return fail(ctx, OD_ERR_ARG, "tuning build (OD_SLIM): exact replay not compiled");
-#else
-    return launch_step<EXTRAS, ExactMath>(ctx, scheme, f64, p);
-#endif
-}
-
 extern "C" int od_step_oceandrift(od_ctx* ctx, const od_step_args* a) {
     if (!ctx || !a) return fail(ctx, OD_ERR_ARG, "od_step_oceandrift: null argument");
     CK(cudaSetDevice(ctx->device));
@@ -1491,12 +1416,8 @@ extern "C" int od_analytic_advect(od_ctx* ctx, const od_analytic_desc* r, const 
     p.env_u = a->d_env_u; p.env_v = a->d_env_v;
     // the analytical sampler has no float32 variant: OD_MATH_FAST keeps its float32 mid-point moves only
     if (a->math == OD_MATH_FAST) return launch_analytic<FastMath>(ctx, a->scheme, a->factor_f64 != 0, p);
-#ifdef OD_SLIM
-    return launch_analytic<SeriesMath>(ctx, a->scheme, a->factor_f64 != 0, p);
-#else
     if (a->math == OD_MATH_SERIES) return launch_analytic<SeriesMath>(ctx, a->scheme, a->factor_f64 != 0, p);
     return launch_analytic<ExactMath>(ctx, a->scheme, a->factor_f64 != 0, p);
-#endif
 }
 
 // ---- output buffer on the device (od_history.cuh) -----------------------------------------------------------
@@ -1529,24 +1450,26 @@ extern "C" int od_history_scatter(od_ctx* ctx, const od_history_args* a) {
 __global__ void __launch_bounds__(256) buoyancy_kernel(const BuoyancyParams p) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const bool d = i < p.n && buoyancy_one(p, i);
-    const unsigned m = __ballot_sync(0xffffffffu, d);
-    if (m && (threadIdx.x & 31) == 0 && p.counter) atomicAdd(p.counter, (unsigned)__popc(m));
+    if (p.counter) tally_flags<1>(p.counter, d);
 }
 
 __global__ void __launch_bounds__(256) bookkeep_kernel(const BookkeepParams p) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    const int f = i < p.n ? bookkeep_one(p, i) : 0;
-    const unsigned m0 = __ballot_sync(0xffffffffu, f & 1), m1 = __ballot_sync(0xffffffffu, f & 2), m2 = __ballot_sync(0xffffffffu, f & 4);
-    if ((threadIdx.x & 31) == 0) {
-        if (m0) atomicAdd(&p.counters[0], (unsigned)__popc(m0));
-        if (m1) atomicAdd(&p.counters[1], (unsigned)__popc(m1));
-        if (m2) atomicAdd(&p.counters[2], (unsigned)__popc(m2));
-    }
+    tally_flags<3>(p.counters, i < p.n ? bookkeep_one(p, i) : 0);
 }
 
 static int counters(od_ctx* ctx) {
     if (!ctx->d_cnt) CK(cudaMalloc(&ctx->d_cnt, 4 * sizeof(unsigned)));
     CK(cudaMemsetAsync(ctx->d_cnt, 0, 4 * sizeof(unsigned), ctx->stream));
+    return OD_OK;
+}
+
+// out[0..k) = the first k counters of the last housekeeping launch (synchronises)
+static int read_counters(od_ctx* ctx, int k, int64_t* out) {
+    unsigned c[4];
+    CK(cudaMemcpyAsync(c, ctx->d_cnt, k * sizeof(unsigned), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    for (int j = 0; j < k; ++j) out[j] = c[j];
     return OD_OK;
 }
 
@@ -1566,13 +1489,7 @@ extern "C" int od_vertical_buoyancy(od_ctx* ctx, const od_buoyancy_args* a) {
     buoyancy_kernel<<<(unsigned)((a->n + 255) / 256), 256, 0, ctx->stream>>>(p);
     CK(cudaGetLastError());
     ctx->launches++;
-    if (a->h_n_deactivated) {
-        unsigned c = 0;
-        CK(cudaMemcpyAsync(&c, ctx->d_cnt, sizeof(c), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        *a->h_n_deactivated = c;
-    }
-    return OD_OK;
+    return a->h_n_deactivated ? read_counters(ctx, 1, a->h_n_deactivated) : OD_OK;
 }
 
 extern "C" int od_bookkeeping(od_ctx* ctx, const od_bookkeep_args* a) {
@@ -1598,13 +1515,7 @@ extern "C" int od_bookkeeping(od_ctx* ctx, const od_bookkeep_args* a) {
     bookkeep_kernel<<<(unsigned)((a->n + 255) / 256), 256, 0, ctx->stream>>>(p);
     CK(cudaGetLastError());
     ctx->launches++;
-    if (a->h_counts) {
-        unsigned c[3] = {0, 0, 0};
-        CK(cudaMemcpyAsync(c, ctx->d_cnt, sizeof(c), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        for (int k = 0; k < 3; ++k) a->h_counts[k] = c[k];
-    }
-    return OD_OK;
+    return a->h_counts ? read_counters(ctx, 3, a->h_counts) : OD_OK;
 }
 
 extern "C" int od_coastline(od_ctx* ctx, const od_coast_args* a) {
@@ -1628,13 +1539,7 @@ extern "C" int od_coastline(od_ctx* ctx, const od_coast_args* a) {
     coast_kernel<<<(unsigned)((a->n + 255) / 256), 256, 0, ctx->stream>>>(p);
     CK(cudaGetLastError());
     ctx->launches++;
-    if (a->h_counts) {
-        unsigned c[4] = {0, 0, 0, 0};
-        CK(cudaMemcpyAsync(c, ctx->d_cnt, sizeof(c), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        for (int k = 0; k < 4; ++k) a->h_counts[k] = c[k];
-    }
-    return OD_OK;
+    return a->h_counts ? read_counters(ctx, 4, a->h_counts) : OD_OK;
 }
 
 extern "C" int od_store_previous(od_ctx* ctx, int64_t n, const double* lon, const double* lat, const int32_t* ids, int32_t id_base,
@@ -1825,13 +1730,7 @@ extern "C" int od_vertical_mixing(od_ctx* ctx, const od_mix_args* a) {
     else mix_kernel<false><<<grid_for(a->n), OD_BLOCK, 0, ctx->stream>>>(p);
     CK(cudaGetLastError());
     ctx->launches++;
-    if (a->seafloor_action == 2 && a->h_n_deactivated) {
-        unsigned c = 0;
-        CK(cudaMemcpyAsync(&c, ctx->d_cnt, sizeof(c), cudaMemcpyDeviceToHost, ctx->stream));
-        CK(cudaStreamSynchronize(ctx->stream));
-        *a->h_n_deactivated = c;
-    }
-    return OD_OK;
+    return a->seafloor_action == 2 && a->h_n_deactivated ? read_counters(ctx, 1, a->h_n_deactivated) : OD_OK;
 }
 
 extern "C" int od_sort_by_cell(od_ctx* ctx, int group, int64_t n, const double* lon, const double* lat, const float* z,
@@ -1850,18 +1749,10 @@ extern "C" int od_sort_by_cell(od_ctx* ctx, int group, int64_t n, const double* 
     p.nty = (g.desc.ny + p.tile - 1) / p.tile;
     const int64_t nbins = 1 + (int64_t)p.ntx * p.nty * g.desc.nz;
     if (nbins >= (1ll << 30)) return fail(ctx, OD_ERR_ARG, "od_sort_by_cell: too many bins");
-    if (ctx->keys_cap < n) {
-        if (ctx->d_keys) cudaFree(ctx->d_keys);
-        ctx->d_keys = nullptr;
-        CK(cudaMalloc(&ctx->d_keys, n * sizeof(int32_t)));
-        ctx->keys_cap = n;
-    }
-    if (ctx->bins_cap < nbins) {
-        if (ctx->d_bins) cudaFree(ctx->d_bins);
-        ctx->d_bins = nullptr;
-        CK(cudaMalloc(&ctx->d_bins, nbins * sizeof(int32_t)));
-        ctx->bins_cap = nbins;
-    }
+    rc = grow(ctx, (void**)&ctx->d_keys, &ctx->keys_cap, n, sizeof(int32_t));
+    if (rc) return rc;
+    rc = grow(ctx, (void**)&ctx->d_bins, &ctx->bins_cap, nbins, sizeof(int32_t));
+    if (rc) return rc;
     CK(cudaMemsetAsync(ctx->d_bins, 0, nbins * sizeof(int32_t), ctx->stream));
     if (p.g.proj_kind) cell_key_kernel<true><<<grid_for(n), OD_BLOCK, 0, ctx->stream>>>(p, ctx->d_keys, ctx->d_bins);
     else cell_key_kernel<false><<<grid_for(n), OD_BLOCK, 0, ctx->stream>>>(p, ctx->d_keys, ctx->d_bins);
@@ -1880,16 +1771,12 @@ extern "C" int od_partition_active(od_ctx* ctx, int64_t n, const int32_t* d_stat
     if (n == 0) return OD_OK;
     CK(cudaSetDevice(ctx->device));
     const int nblocks = (int)((n + OD_PART_BLOCK - 1) / OD_PART_BLOCK);
-    if (ctx->bins_cap < nblocks + 1) {
-        if (ctx->d_bins) cudaFree(ctx->d_bins);
-        ctx->d_bins = nullptr;
-        CK(cudaMalloc(&ctx->d_bins, (size_t)(nblocks + 1) * sizeof(int32_t)));
-        ctx->bins_cap = nblocks + 1;
-    }
+    int rc = grow(ctx, (void**)&ctx->d_bins, &ctx->bins_cap, nblocks + 1, sizeof(int32_t));
+    if (rc) return rc;
     CK(cudaMemsetAsync(ctx->d_bins + nblocks, 0, sizeof(int32_t), ctx->stream));
     partition_count_kernel<<<nblocks, OD_PART_BLOCK, 0, ctx->stream>>>(n, d_status, ctx->d_bins);
-    int rcs = scan_exclusive(ctx, ctx->d_bins, nblocks + 1);                       // exclusive; last entry = total
-    if (rcs) return rcs;
+    rc = scan_exclusive(ctx, ctx->d_bins, nblocks + 1);                            // exclusive; last entry = total
+    if (rc) return rc;
     int32_t total = 0;
     CK(cudaMemcpyAsync(&total, ctx->d_bins + nblocks, sizeof(int32_t), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -1956,16 +1843,12 @@ extern "C" int od_pack_by_owner(od_ctx* ctx, const od_pack_args* a) {
     }
     p.nblocks = (int)((a->n + OD_PACK_BLOCK - 1) / OD_PACK_BLOCK);
     const int64_t nbins = (int64_t)p.nblocks * a->world + 1;           // (+1: the grand total lands behind the table)
-    if (ctx->bins_cap < nbins) {
-        if (ctx->d_bins) cudaFree(ctx->d_bins);
-        ctx->d_bins = nullptr;
-        CK(cudaMalloc(&ctx->d_bins, nbins * sizeof(int32_t)));
-        ctx->bins_cap = nbins;
-    }
+    int rc = grow(ctx, (void**)&ctx->d_bins, &ctx->bins_cap, nbins, sizeof(int32_t));
+    if (rc) return rc;
     CK(cudaMemsetAsync(ctx->d_bins + (nbins - 1), 0, sizeof(int32_t), ctx->stream));
     owner_count_kernel<<<p.nblocks, OD_PACK_BLOCK, 0, ctx->stream>>>(p, ctx->d_bins);
     ctx->launches++;
-    int rc = scan_exclusive(ctx, ctx->d_bins, (int)nbins);
+    rc = scan_exclusive(ctx, ctx->d_bins, (int)nbins);
     if (rc) return rc;
     owner_pack_kernel<<<p.nblocks, OD_PACK_BLOCK, 0, ctx->stream>>>(p, ctx->d_bins, (unsigned char*)a->d_records, a->d_perm);
     CK(cudaGetLastError());

@@ -11,6 +11,19 @@
 #error "od_step.cu is compiled once per arithmetic mode and step variant: -DOD_STEP_MATH=... -DOD_STEP_EXTRAS=0|1|2"
 #endif
 
+// Calls f(std::integral_constant<int, SCHEME>, std::bool_constant<F64>) for the advection scheme (OD_EULER, OD_RK2, else
+// OD_RK4) and the factor dtype: every launcher instantiates its kernel for all six combinations through this.
+template <class F>
+static void dispatch_scheme(int scheme, bool f64, F&& f) {
+    auto by_dtype = [&](auto s) {
+        if (f64) f(s, std::bool_constant<true>{});
+        else f(s, std::bool_constant<false>{});
+    };
+    if (scheme == OD_EULER) by_dtype(std::integral_constant<int, 0>{});
+    else if (scheme == OD_RK2) by_dtype(std::integral_constant<int, 1>{});
+    else by_dtype(std::integral_constant<int, 2>{});
+}
+
 template <int SCHEME, bool F64, int EXTRAS, class MATH>
 __global__ void __launch_bounds__(OD_BLOCK, OD_STEP_MINB) step_kernel(const __grid_constant__ StepParams p) {
     __shared__ LevelsSmem lv;
@@ -142,15 +155,9 @@ template <int EXTRAS, class MATH>
 int launch_step_tiled(od_ctx* ctx, int scheme, bool f64, const StepParams& p, const PairEntry* pe) {
     const int grid = grid_for(p.n);
     cudaStream_t s = ctx->stream;
-#define OD_LAUNCHT(S, F) step_tiled_kernel<S, F, EXTRAS, MATH><<<grid, OD_BLOCK, 0, s>>>(p, pe->tmap, pe->tex)
-#ifdef OD_SLIM
-    return fail(ctx, OD_ERR_ARG, "tuning build (OD_SLIM): tiled kernels not compiled");
-#else
-    if (scheme == OD_EULER) { if (f64) OD_LAUNCHT(0, true); else OD_LAUNCHT(0, false); }
-    else if (scheme == OD_RK2) { if (f64) OD_LAUNCHT(1, true); else OD_LAUNCHT(1, false); }
-    else { if (f64) OD_LAUNCHT(2, true); else OD_LAUNCHT(2, false); }
-#endif
-#undef OD_LAUNCHT
+    dispatch_scheme(scheme, f64, [&](auto S, auto F) {
+        step_tiled_kernel<decltype(S)::value, decltype(F)::value, EXTRAS, MATH><<<grid, OD_BLOCK, 0, s>>>(p, pe->tmap, pe->tex);
+    });
     CK(cudaGetLastError());
     ctx->launches++;
     return OD_OK;
@@ -160,11 +167,9 @@ template <int E, class MATH>
 int launch_step_chain(od_ctx* ctx, int scheme, bool f64, const StepParams& p) {
     const int grid = grid_for(p.n);
     cudaStream_t s = ctx->stream;
-#define OD_LAUNCHC(S, F) step_chain_kernel<S, F, E, MATH><<<grid, OD_BLOCK, 0, s>>>(p)
-    if (scheme == OD_EULER) { if (f64) OD_LAUNCHC(0, true); else OD_LAUNCHC(0, false); }
-    else if (scheme == OD_RK2) { if (f64) OD_LAUNCHC(1, true); else OD_LAUNCHC(1, false); }
-    else { if (f64) OD_LAUNCHC(2, true); else OD_LAUNCHC(2, false); }
-#undef OD_LAUNCHC
+    dispatch_scheme(scheme, f64, [&](auto S, auto F) {
+        step_chain_kernel<decltype(S)::value, decltype(F)::value, E, MATH><<<grid, OD_BLOCK, 0, s>>>(p);
+    });
     CK(cudaGetLastError());
     ctx->launches++;
     return OD_OK;
@@ -187,25 +192,14 @@ int launch_step(od_ctx* ctx, int scheme, bool f64, const StepParams& p) {
             return OD_OK;
         }
     }
-#ifdef OD_SLIM
-    // tuning builds: only the bench's instantiations (RK4, float64 factor, no reader chain) are compiled
-    if (p.n_chain > 0 || scheme != OD_RK4 || !f64) return fail(ctx, OD_ERR_ARG, "tuning build (OD_SLIM): kernel variant not compiled");
-    step_kernel<2, true, EXTRAS, MATH><<<grid, OD_BLOCK, 0, s>>>(p);
-    CK(cudaGetLastError());
-    ctx->launches++;
-    return OD_OK;
-#else
     const bool general = p.n_chain > 0 || p.cs.g.proj_kind != 0 || (EXTRAS != 0 && ((p.wind_on && p.gwind.proj_kind != 0) || (p.w_on && p.gw.proj_kind != 0)));
     if (general) return launch_step_chain<EXTRAS == 0 ? 0 : 1, MATH>(ctx, scheme, f64, p);
-#define OD_LAUNCH(S, F) step_kernel<S, F, EXTRAS, MATH><<<grid, OD_BLOCK, 0, s>>>(p)
-    if (scheme == OD_EULER) { if (f64) OD_LAUNCH(0, true); else OD_LAUNCH(0, false); }
-    else if (scheme == OD_RK2) { if (f64) OD_LAUNCH(1, true); else OD_LAUNCH(1, false); }
-    else { if (f64) OD_LAUNCH(2, true); else OD_LAUNCH(2, false); }
-#undef OD_LAUNCH
+    dispatch_scheme(scheme, f64, [&](auto S, auto F) {
+        step_kernel<decltype(S)::value, decltype(F)::value, EXTRAS, MATH><<<grid, OD_BLOCK, 0, s>>>(p);
+    });
     CK(cudaGetLastError());
     ctx->launches++;
     return OD_OK;
-#endif
 }
 
 // ---- analytical reader on a projected plane (od_analytic.cuh) ---------------------------------------------
@@ -220,16 +214,9 @@ template <class MATH>
 int launch_analytic(od_ctx* ctx, int scheme, bool f64, const AnalyticStepParams& p) {
     const int grid = grid_for(p.n);
     cudaStream_t s = ctx->stream;
-#define OD_LAUNCHA(S, F) analytic_step_kernel<S, F, MATH><<<grid, OD_BLOCK, 0, s>>>(p)
-#ifdef OD_SLIM
-    if (scheme != OD_RK4 || !f64) return fail(ctx, OD_ERR_ARG, "tuning build (OD_SLIM): kernel variant not compiled");
-    OD_LAUNCHA(2, true);
-#else
-    if (scheme == OD_EULER) { if (f64) OD_LAUNCHA(0, true); else OD_LAUNCHA(0, false); }
-    else if (scheme == OD_RK2) { if (f64) OD_LAUNCHA(1, true); else OD_LAUNCHA(1, false); }
-    else { if (f64) OD_LAUNCHA(2, true); else OD_LAUNCHA(2, false); }
-#endif
-#undef OD_LAUNCHA
+    dispatch_scheme(scheme, f64, [&](auto S, auto F) {
+        analytic_step_kernel<decltype(S)::value, decltype(F)::value, MATH><<<grid, OD_BLOCK, 0, s>>>(p);
+    });
     CK(cudaGetLastError());
     ctx->launches++;
     return OD_OK;
