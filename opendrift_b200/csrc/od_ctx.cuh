@@ -21,8 +21,11 @@ using namespace od;
 #ifndef OD_STEP_MINB
 #define OD_STEP_MINB 8
 #endif
+// The specialised step kernel (od_spec.cuh) at 6 blocks per SM: 80 registers, 24 warps/SM.  At 8 blocks (64 registers) it
+// spilled 132-176 B per thread; with the wind move (EXTRAS = 1) it took 20 % longer, and steps that start or end on a reader
+// time 3-7 % longer (DESIGN.md §5).
 #ifndef OD_SPEC_MINB
-#define OD_SPEC_MINB OD_STEP_MINB
+#define OD_SPEC_MINB 6
 #endif
 
 // ------------------------------------------------------------------------------------------------
