@@ -387,6 +387,13 @@ typedef struct od_stokes_args {
 
 int od_stokes_drift(od_ctx* ctx, const od_stokes_args* a);
 
+/* drift:use_tabularised_stokes_drift (basemodel/environment.py:844-863, physics_methods.py:488-568): Stokes drift and significant
+ * wave height from the float32 wind, in place.  ws = sqrt(x^2 + y^2) (float64, capped at 30); d_us / d_vs = float32(wind * wf) with
+ * wf = np.polyval(h_wf, ws) in float64; d_hs = float32(np.polyval(h_hs, ws)).  h_wf / h_hs are host arrays of 1..8 coefficients,
+ * highest power first.  d_us and d_vs (both or neither) and d_hs may be NULL: that output is not written. */
+int od_stokes_parameterised(od_ctx* ctx, int64_t n, const float* d_xwind, const float* d_ywind, const double* h_wf, int32_t n_wf,
+                            const double* h_hs, int32_t n_hs, float* d_us, float* d_vs, float* d_hs);
+
 /* ---- vertical turbulent mixing ----------------------------------------------------------------
  * OceanDrift.vertical_mixing (models/oceandrift.py:397-571) with diffusivity from the environment profiles of
  * a 3-D one-component group: all int(dt/dt_mix) inner random-walk iterations in one launch.  Positions are

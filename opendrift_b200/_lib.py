@@ -200,6 +200,7 @@ SYMBOLS = {
     'od_analytic_advect': (C.c_int, [_P, C.POINTER(AnalyticDesc), C.POINTER(AnalyticAdvectArgs)]),
     'od_minmax_f32': (C.c_int, [_P, C.c_int64, _P, _P, C.POINTER(C.c_float), C.POINTER(C.c_float)]),
     'od_stokes_drift': (C.c_int, [_P, C.POINTER(StokesArgs)]),
+    'od_stokes_parameterised': (C.c_int, [_P, C.c_int64, _P, _P, _P, C.c_int32, _P, C.c_int32, _P, _P, _P]),
     'od_vertical_mixing': (C.c_int, [_P, C.POINTER(MixArgs)]),
     'od_vertical_buoyancy': (C.c_int, [_P, C.POINTER(BuoyancyArgs)]),
     'od_bookkeeping': (C.c_int, [_P, C.POINTER(BookkeepArgs)]),

@@ -729,6 +729,11 @@ __global__ void __launch_bounds__(256) minmax_kernel(int64_t n, const float* __r
     }
 }
 
+__global__ void __launch_bounds__(256) stokes_tab_kernel(const StokesTabParams p) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += (int64_t)gridDim.x * blockDim.x)
+        stokes_tab_one(p, i);
+}
+
 // ---- particle ordering ---------------------------------------------------------------------------
 struct SortParams {
     GroupGeom g;
@@ -1671,6 +1676,27 @@ extern "C" int od_stokes_drift(od_ctx* ctx, const od_stokes_args* a) {
     p.sw_dir = a->d_swell_dir; p.sw_period = a->d_swell_period; p.sw_hs = a->d_swell_hs;
     p.ws_dir = a->d_windsea_dir; p.ws_period = a->d_windsea_period; p.ws_hs = a->d_windsea_hs;
     stokes_kernel<<<grid_for(a->n), OD_BLOCK, 0, ctx->stream>>>(p);
+    CK(cudaGetLastError());
+    ctx->launches++;
+    return OD_OK;
+}
+
+extern "C" int od_stokes_parameterised(od_ctx* ctx, int64_t n, const float* xwind, const float* ywind, const double* wf_coef,
+                                       int32_t n_wf, const double* hs_coef, int32_t n_hs, float* us, float* vs, float* hs) {
+    if (!ctx || n < 0 || (!us) != (!vs) || (!us && !hs) || (n > 0 && (!xwind || !ywind)))
+        return fail(ctx, OD_ERR_ARG, "od_stokes_parameterised: bad arguments");
+    if ((us && (!wf_coef || n_wf < 1 || n_wf > OD_TAB_MAX_COEF)) || (hs && (!hs_coef || n_hs < 1 || n_hs > OD_TAB_MAX_COEF)))
+        return fail(ctx, OD_ERR_ARG, "od_stokes_parameterised: 1 to 8 coefficients per polynomial");
+    if (n == 0) return OD_OK;
+    CK(cudaSetDevice(ctx->device));
+    StokesTabParams p;
+    memset(&p, 0, sizeof(p));
+    p.n = n; p.xwind = xwind; p.ywind = ywind; p.us = us; p.vs = vs; p.hs = hs;
+    if (us) { p.n_wf = n_wf; memcpy(p.wf, wf_coef, sizeof(double) * n_wf); }
+    if (hs) { p.n_hs = n_hs; memcpy(p.hsc, hs_coef, sizeof(double) * n_hs); }
+    int64_t blocks = (n + 255) / 256;
+    if (blocks > (int64_t)ctx->sm_count * 8) blocks = (int64_t)ctx->sm_count * 8;
+    stokes_tab_kernel<<<(unsigned)blocks, 256, 0, ctx->stream>>>(p);
     CK(cudaGetLastError());
     ctx->launches++;
     return OD_OK;

@@ -174,4 +174,50 @@ OD_HD void stokes_particle(const StokesParams& p, int64_t i) {
     p.lat[i] = la;
 }
 
+// ---- drift:use_tabularised_stokes_drift: Stokes drift and Hs from the wind (physics_methods.py:488-568) ----------------------------
+// wave_stokes_drift_parameterised / wave_significant_height_parameterised in the dtype flow NumPy gives them.  The wind arrives as
+// fields of the reference's masked environment array, and np.ma.power squares a float32 masked array in float64 (the exponent
+// becomes a 0-d int64 array, which is not a weak scalar):
+//   ws = sqrt(x^2 + y^2) in float64 from the float32 wind (each square exact), ws > 30 -> 30 (NaN stays);
+//   np.polyval(c, ws): y = 0*ws + c[0] is c[0] (NaN for a NaN ws), then y = y*ws + c[k] in float64;
+//   us = float32(float64(x) * wf), vs likewise; Hs = float32(polyval).  No fused multiply-add anywhere.
+// The coefficients are np.polyfit of the reference's tables, computed by the host.
+#define OD_TAB_MAX_COEF 8
+
+struct StokesTabParams {
+    int64_t n;
+    const float* xwind;
+    const float* ywind;
+    float* us;                   // NULL: the Stokes drift is not replaced
+    float* vs;
+    float* hs;                   // NULL: Hs is not replaced
+    int32_t n_wf, n_hs;          // number of coefficients (polynomial order + 1)
+    double wf[OD_TAB_MAX_COEF];  // highest power first, as np.polyfit returns them
+    double hsc[OD_TAB_MAX_COEF];
+};
+
+OD_HD double tab_polyval(const double* c, int32_t nc, double ws) {
+    if (ws != ws) return ws;
+    double y = c[0];
+    for (int32_t k = 1; k < nc; ++k) y = OD_DADD(OD_DMUL(y, ws), c[k]);
+    return y;
+}
+
+OD_HD void stokes_tab_one(const StokesTabParams& p, int64_t i) {
+    const double xw = (double)p.xwind[i], yw = (double)p.ywind[i];
+    const double s2 = OD_DADD(OD_DMUL(xw, xw), OD_DMUL(yw, yw));
+#if defined(__CUDA_ARCH__)
+    double ws = __dsqrt_rn(s2);
+#else
+    double ws = sqrt(s2);
+#endif
+    if (ws > 30.0) ws = 30.0;
+    if (p.us) {
+        const double wf = tab_polyval(p.wf, p.n_wf, ws);
+        p.us[i] = (float)OD_DMUL(xw, wf);
+        p.vs[i] = (float)OD_DMUL(yw, wf);
+    }
+    if (p.hs) p.hs[i] = (float)tab_polyval(p.hsc, p.n_hs, ws);
+}
+
 }  // namespace od

@@ -943,6 +943,20 @@ class Engine:
         a.dt, a.hs_mode, a.profile = float(dt), int(hs_mode), self.PROFILES[profile]
         self._check(self.lib.od_stokes_drift(self.ctx, C.byref(a)))
 
+    def stokes_parameterised(self, xwind, ywind, wf_coef, hs_coef, us=None, vs=None, hs=None):
+        """drift:use_tabularised_stokes_drift: writes float32(wind * np.polyval(wf_coef, ws)) into us / vs and
+        float32(np.polyval(hs_coef, ws)) into hs, in place (float32 device tensors; None: not written).  ws is the wind speed,
+        in float64, capped at 30 m/s; the coefficients are np.polyfit's, highest power first."""
+        torch = self.torch
+        assert xwind.dtype == ywind.dtype == torch.float32
+        outs = [t for t in (us, vs, hs) if t is not None]
+        assert all(t.dtype == torch.float32 and t.numel() == xwind.numel() for t in outs)
+        cw = np.ascontiguousarray(wf_coef if us is not None else [], dtype=np.float64)
+        ch = np.ascontiguousarray(hs_coef if hs is not None else [], dtype=np.float64)
+        self._check(self.lib.od_stokes_parameterised(self.ctx, xwind.numel(), _ptr(xwind), _ptr(ywind),
+                                                     cw.ctypes.data_as(C.c_void_p), len(cw), ch.ctypes.data_as(C.c_void_p),
+                                                     len(ch), _ptr(us), _ptr(vs), _ptr(hs)))
+
     MIX_MODELS = {'environment': _lib.OD_MIX_ENVIRONMENT, 'windspeed_Large1994': _lib.OD_MIX_LARGE1994,
                   'windspeed_Sundby1983': _lib.OD_MIX_SUNDBY1983, 'constant': _lib.OD_MIX_CONSTANT}
 

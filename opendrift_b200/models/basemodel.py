@@ -1011,7 +1011,7 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
             raise NotImplementedError('file export is outside the GPU hot path; read o.history / o.elements')
         if self.num_elements_scheduled() == 0:
             raise ValueError('Please seed elements before starting a run.')
-        for key in ('drift:water_column_stretching', 'drift:use_tabularised_stokes_drift', 'vertical_mixing:TSprofiles'):
+        for key in ('drift:water_column_stretching', 'vertical_mixing:TSprofiles'):
             if key in self._config and self.get_config(key):
                 raise NotImplementedError('%s = True is not on the GPU path' % key)
         from .. import _lib
@@ -1085,6 +1085,10 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
             # the reference's previous-step store writes newly released elements at their positions in the whole element array
             # (update_previous_state :651-653); a shard sees only its own positions
             raise NotImplementedError('drift:vertical_advection_correction = True is not on the distributed GPU path')
+        if self._dist is not None and self.get_config('drift:use_tabularised_stokes_drift', False):
+            # the reference decides whether to replace the Stokes drift and Hs from their maxima over the whole element array;
+            # a shard sees only its own elements
+            raise NotImplementedError('drift:use_tabularised_stokes_drift = True is not on the distributed GPU path')
         self.shard = None
         if self._dist is not None and self.get_config('gpu:shard') == 'index':
             n_all = int(self.num_elements_total())

@@ -20,6 +20,34 @@ logger = logging.getLogger('opendrift_b200')
 # variables a StructuredReader serves without time interpolation (readers/basereader/structured.py:224-229)
 STATIC_VARIABLES = ('sea_floor_depth_below_sea_level', 'land_binary_mask')
 
+# drift:use_tabularised_stokes_drift (physics_methods.py:488-568): per fetch (m), the tabulated Stokes drift factor wf
+# (Stokes drift = wf * wind) and significant wave height (m) at wind speeds 0, 1, ..., 29 m/s, and the order of the
+# polynomial fitted to the Stokes drift factor (the height is fitted with a straight line)
+STOKES_TABLES = {
+    '5000': (3, (0.0173, 0.0160, 0.0152, 0.0145, 0.0139, 0.0135, 0.0132, 0.0129, 0.0126, 0.0124, 0.0122, 0.0121, 0.0119, 0.0118,
+                 0.0117, 0.0116, 0.0114, 0.0113, 0.0112, 0.0112, 0.0111, 0.0110, 0.0109, 0.0109, 0.0108, 0.0107, 0.0106, 0.0106,
+                 0.0106, 0.0105),
+             (0.030, 0.077, 0.124, 0.170, 0.216, 0.263, 0.311, 0.360, 0.409, 0.459, 0.509, 0.560, 0.612, 0.664, 0.716, 0.771, 0.823,
+              0.876, 0.932, 0.987, 1.041, 1.095, 1.152, 1.210, 1.265, 1.319, 1.375, 1.434, 1.494, 1.552)),
+    '25000': (6, (0.0173, 0.0197, 0.0201, 0.0185, 0.0181, 0.0176, 0.0171, 0.0167, 0.0164, 0.0160, 0.0158, 0.0155, 0.0153, 0.0151,
+                  0.0149, 0.0147, 0.0146, 0.0144, 0.0143, 0.0142, 0.0140, 0.0139, 0.0138, 0.0137, 0.0136, 0.0135, 0.0135, 0.0134,
+                  0.0133, 0.0132),
+              (0.030, 0.122, 0.251, 0.336, 0.442, 0.546, 0.650, 0.753, 0.856, 0.959, 1.063, 1.168, 1.273, 1.379, 1.486, 1.593, 1.702,
+               1.811, 1.920, 2.030, 2.142, 2.254, 2.366, 2.478, 2.592, 2.707, 2.822, 2.936, 3.051, 3.166)),
+    '50000': (6, (0.0173, 0.0197, 0.0210, 0.0216, 0.0201, 0.0194, 0.0190, 0.0186, 0.0183, 0.0179, 0.0176, 0.0173, 0.0171, 0.0168,
+                  0.0166, 0.0164, 0.0162, 0.0160, 0.0159, 0.0157, 0.0156, 0.0155, 0.0153, 0.0152, 0.0151, 0.0150, 0.0149, 0.0148,
+                  0.0147, 0.0146),
+              (0.030, 0.122, 0.274, 0.474, 0.591, 0.724, 0.873, 1.021, 1.168, 1.314, 1.460, 1.606, 1.752, 1.898, 2.045, 2.192, 2.340,
+               2.489, 2.639, 2.789, 2.940, 3.092, 3.244, 3.397, 3.551, 3.706, 3.862, 4.017, 4.173, 4.330)),
+}
+
+
+def stokes_coefficients(fetch):
+    """(Stokes drift factor, significant wave height) polynomial coefficients for a fetch, highest power first: np.polyfit of
+    the tables against the wind speed, in float64."""
+    order, wf, hs = STOKES_TABLES[str(fetch)]
+    return np.polyfit(range(len(wf)), wf, order), np.polyfit(range(len(hs)), hs, 1)
+
 
 class Environment:
     def __init__(self, required_variables, config):
@@ -30,6 +58,7 @@ class Environment:
         self.discarded_readers = {}
         self.__finalized__ = False
         self._engine = None
+        self._stokes_coef = None          # (wf, Hs) coefficients while drift:use_tabularised_stokes_drift is on
 
     # -- registry (environment.py:267-330) -------------------------------------------------------
     def add_reader(self, readers, variables=None, first=False):
@@ -60,6 +89,9 @@ class Environment:
                 r.set_buffer_size(max_speed=ms['value'])             # environment.py:402
             if hasattr(r, 'bind'):
                 r.bind(engine, fallback={v: self.fallback(v) for v in r.variables})
+        self._stokes_coef = None
+        if self._config._config.get('drift:use_tabularised_stokes_drift', {}).get('value') is True:
+            self._stokes_coef = stokes_coefficients(self._config.get_config('drift:tabularised_stokes_drift_fetch'))
         self.__finalized__ = True
 
     def subblock_readers(self):
@@ -219,10 +251,36 @@ class Environment:
                     if fb is not None:
                         t = torch.where(torch.isfinite(t), t, torch.full_like(t, float(fb)))
                     out[nm] = t
+        if self._stokes_coef is not None and 'x_wind' in out:
+            self._parameterise_stokes(out)
         missing = torch.zeros(n, dtype=torch.bool, device=eng.device)
         for v in variables:
             missing |= ~torch.isfinite(out[v])
         return out, missing
+
+    def _parameterise_stokes(self, out):
+        """drift:use_tabularised_stokes_drift (environment.py:844-863), after the fallbacks and before any uncertainty draw: both
+        Stokes components become wind * wf when the maximum of each is exactly 0 over the call's elements (a reader whose values
+        are all <= 0 with one exact 0 included), and Hs the fitted height when its maximum is 0.  A variable the call did not
+        request is left out (the reference has no field to write it into and stops)."""
+        eng, torch = self._engine, self._engine.torch
+        sx, sy = 'sea_surface_wave_stokes_drift_x_velocity', 'sea_surface_wave_stokes_drift_y_velocity'
+        hs = 'sea_surface_wave_significant_height'
+        if 'y_wind' not in out:
+            return
+        stokes = sx in out and sy in out and eng.minmax(out[sx])[1] == 0 and eng.minmax(out[sy])[1] == 0
+        height = hs in out and eng.minmax(out[hs])[1] == 0
+        if not (stokes or height):
+            return
+        # fresh outputs: a sampled tensor may be shared with another variable or a reader
+        us = torch.empty_like(out['x_wind']) if stokes else None
+        vs = torch.empty_like(out['x_wind']) if stokes else None
+        h = torch.empty_like(out['x_wind']) if height else None
+        eng.stokes_parameterised(out['x_wind'], out['y_wind'], self._stokes_coef[0], self._stokes_coef[1], us, vs, h)
+        if stokes:
+            out[sx], out[sy] = us, vs
+        if height:
+            out[hs] = h
 
     # -- host face (the reference signature) ---------------------------------------------------------
     def get_environment(self, variables, time, lon, lat, z, profiles=None, profiles_depth=None, element_ID=None):

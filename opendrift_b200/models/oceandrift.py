@@ -83,9 +83,13 @@ class OceanDrift(OpenDriftSimulation):
                                                                    'sea surface height from the vertical water velocity '
                                                                    '(refused in distributed runs).'},
             'drift:use_tabularised_stokes_drift': {'type': 'bool', 'default': False, 'level': CONFIG_LEVEL_BASIC,
-                                                   'description': 'Accepted with the reference\'s default; True is refused at run().'},
+                                                   'description': 'If True, Stokes drift is estimated from wind based on look-up-tables '
+                                                                  'for given fetch (drift:tabularised_stokes_drift_fetch), where no '
+                                                                  'reader provides it; also the significant wave height '
+                                                                  '(refused in distributed runs).'},
             'drift:tabularised_stokes_drift_fetch': {'type': 'enum', 'enum': ['5000', '25000', '50000'], 'default': '25000',
-                                                     'level': CONFIG_LEVEL_ADVANCED, 'description': 'Only used with tabularised Stokes drift.'},
+                                                     'level': CONFIG_LEVEL_ADVANCED,
+                                                     'description': 'The fetch length (m) when using tabularised Stokes drift.'},
             'vertical_mixing:TSprofiles': {'type': 'bool', 'default': False, 'level': CONFIG_LEVEL_ADVANCED,
                                            'description': 'Accepted with the reference\'s default; True is refused at run().'},
             'gpu:rng': {'type': 'enum', 'enum': ['numpy', 'philox'], 'default': 'numpy', 'level': CONFIG_LEVEL_ADVANCED,
@@ -437,9 +441,10 @@ class OceanDrift(OpenDriftSimulation):
         # Stokes drift moves between wind drift and the random walk: when it is active its start-of-step samples
         # are taken first, the fused kernel does current + wind (+ w), then the Stokes and diffusion launches follow
         stokes_inp = None
-        if self.get_config('drift:stokes_drift') and any(
+        if self.get_config('drift:stokes_drift') and (self.get_config('drift:use_tabularised_stokes_drift') or any(
                 self.env.priority_list.get(v) or (self.env.constant(v) or 0) != 0
-                for v in ('sea_surface_wave_stokes_drift_x_velocity', 'sea_surface_wave_stokes_drift_y_velocity')):
+                for v in ('sea_surface_wave_stokes_drift_x_velocity', 'sea_surface_wave_stokes_drift_y_velocity'))):
+            # (with drift:use_tabularised_stokes_drift the Stokes drift may come from the wind: _stokes_inputs samples it)
             stokes_inp = self._stokes_inputs()
         split_diffusion = stokes_inp is not None and D != 0
         n = len(el)
