@@ -453,6 +453,20 @@ typedef struct od_mix_args {
 
 int od_vertical_mixing(od_ctx* ctx, const od_mix_args* a);
 
+/* SedimentDrift (models/sedimentdrift.py): od_vertical_mixing with bottom_interaction (:108-116) in every inner iteration.  After
+ * the sea floor, an element at or below Zmin whose moving is 1 settles: moving = 0 for the remaining iterations.  Here a->d_moving
+ * and a->d_status are only read (a->d_moving_out is not used) and nothing of the elements is modified in place: every element's
+ * moving goes to d_moving_out and, with seafloor_action 2, its status to d_status_out.  The reference settles elements only in
+ * iterations where some element of the whole array is below Zmin before the lift; an element that ends an iteration exactly at
+ * Zmin, moving, without having been below itself cannot be decided here.  It is left moving and counted in *h_undecided; a
+ * non-zero count means the result is to be discarded and the step's mixing redone with the decision taken over all elements.
+ * h_undecided (required) and a->h_n_deactivated are read back together (synchronises). */
+int od_vertical_mixing_settle(od_ctx* ctx, const od_mix_args* a, int32_t* d_moving_out, int32_t* d_status_out, int64_t* h_undecided);
+
+/* SedimentDrift.resuspension (models/sedimentdrift.py:118-126): where float32 sqrt(u*u + v*v) > threshold (a float32 comparison) and
+ * moving == 0, moving = 1 and z += 0.01 in z's dtype (float64 when z_f64, else float32).  u, v: the step's float32 current. */
+int od_resuspend(od_ctx* ctx, int64_t n, const float* d_u, const float* d_v, float threshold, int32_t* d_moving, void* d_z, int32_t z_f64);
+
 /* ---- analytical readers on a projected plane ---------------------------------------------------------
  * BASELINE configs[0]: opendrift/readers/reader_double_gyre.py (a ContinuousReader, basereader/continuous.py:9-48) on the
  * spherical stereographic plane its constructor asks pyproj for (reader_double_gyre.py:27-31).  The reader chain of

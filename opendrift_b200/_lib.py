@@ -202,6 +202,8 @@ SYMBOLS = {
     'od_stokes_drift': (C.c_int, [_P, C.POINTER(StokesArgs)]),
     'od_stokes_parameterised': (C.c_int, [_P, C.c_int64, _P, _P, _P, C.c_int32, _P, C.c_int32, _P, _P, _P]),
     'od_vertical_mixing': (C.c_int, [_P, C.POINTER(MixArgs)]),
+    'od_vertical_mixing_settle': (C.c_int, [_P, C.POINTER(MixArgs), _P, _P, C.POINTER(C.c_int64)]),
+    'od_resuspend': (C.c_int, [_P, C.c_int64, _P, _P, C.c_float, _P, _P, C.c_int32]),
     'od_vertical_buoyancy': (C.c_int, [_P, C.POINTER(BuoyancyArgs)]),
     'od_bookkeeping': (C.c_int, [_P, C.POINTER(BookkeepArgs)]),
     'od_coastline': (C.c_int, [_P, C.POINTER(CoastArgs)]),

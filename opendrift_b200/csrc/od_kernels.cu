@@ -682,6 +682,26 @@ __global__ void __launch_bounds__(OD_BLOCK) mix_kernel(const MixParams p) {
     mix_particle<PROJ>(p, i, xs, xy);
 }
 
+template <bool PROJ>
+__global__ void __launch_bounds__(OD_BLOCK) mix_settle_kernel(const MixParams p, const SettleParams st) {
+    __shared__ double xs[OD_MAX_LEVELS];
+    __shared__ double xy[OD_MAX_LEVELS];
+    for (int i = threadIdx.x; p.model == 0 && i < p.g.nz; i += blockDim.x) {
+        xs[i] = p.xs[i];
+        xy[i] = p.xy[i];
+    }
+    __syncthreads();
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= p.n) return;
+    mix_particle<PROJ, true>(p, i, xs, xy, &st);
+}
+
+__global__ void __launch_bounds__(256) resuspend_kernel(int64_t n, const float* __restrict__ u, const float* __restrict__ v,
+                                                        float threshold, int32_t* __restrict__ moving, void* __restrict__ z, int32_t z_f64) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        resuspend_one(i, u, v, threshold, moving, z, z_f64);
+}
+
 // ---- Leeway -------------------------------------------------------------------------------------------
 template <bool PROJ>
 __global__ void __launch_bounds__(OD_BLOCK) leeway_kernel(const LeewayParams p) {
@@ -1702,7 +1722,8 @@ extern "C" int od_stokes_parameterised(od_ctx* ctx, int64_t n, const float* xwin
     return OD_OK;
 }
 
-extern "C" int od_vertical_mixing(od_ctx* ctx, const od_mix_args* a) {
+// od_vertical_mixing, and with st its settling variant (od_vertical_mixing_settle)
+static int mix_launch(od_ctx* ctx, const od_mix_args* a, const SettleParams* st, int64_t* h_undecided) {
     if (!ctx || !a) return fail(ctx, OD_ERR_ARG, "od_vertical_mixing: null argument");
     if (a->n < 0 || a->ntimes < 0 || (a->n > 0 && (!a->d_lon || !a->d_lat || !a->d_z_in || !a->d_z_out)))
         return fail(ctx, OD_ERR_ARG, "od_vertical_mixing: bad arguments");
@@ -1745,18 +1766,62 @@ extern "C" int od_vertical_mixing(od_ctx* ctx, const od_mix_args* a) {
     p.seafloor_action = a->seafloor_action; p.seafloor_code = a->seafloor_code; p.status = a->d_status; p.moving_out = a->d_moving_out;
     p.iter0 = a->iter0; p.skip_surface_stick = a->skip_surface_stick;
     if (a->h_n_deactivated) *a->h_n_deactivated = 0;
-    if (a->seafloor_action < 0 || a->seafloor_action > 2 || (a->seafloor_action == 2 && (!a->d_status || !a->d_moving_out)))
+    if (a->seafloor_action < 0 || a->seafloor_action > 2 || (a->seafloor_action == 2 && (!a->d_status || !(st ? st->status_out : a->d_moving_out))))
         return fail(ctx, OD_ERR_ARG, "od_vertical_mixing: bad sea-floor action");
-    if (a->seafloor_action == 2) {
+    if (a->seafloor_action == 2 || st) {
         int rc = counters(ctx);
         if (rc) return rc;
         p.counter = ctx->d_cnt;
     }
-    if (p.g.proj_kind) mix_kernel<true><<<grid_for(a->n), OD_BLOCK, 0, ctx->stream>>>(p);
-    else mix_kernel<false><<<grid_for(a->n), OD_BLOCK, 0, ctx->stream>>>(p);
+    if (st) {
+        SettleParams s = *st;
+        s.undecided = ctx->d_cnt + 1;
+        if (p.g.proj_kind) mix_settle_kernel<true><<<grid_for(a->n), OD_BLOCK, 0, ctx->stream>>>(p, s);
+        else mix_settle_kernel<false><<<grid_for(a->n), OD_BLOCK, 0, ctx->stream>>>(p, s);
+    } else if (p.g.proj_kind) {
+        mix_kernel<true><<<grid_for(a->n), OD_BLOCK, 0, ctx->stream>>>(p);
+    } else {
+        mix_kernel<false><<<grid_for(a->n), OD_BLOCK, 0, ctx->stream>>>(p);
+    }
     CK(cudaGetLastError());
     ctx->launches++;
+    if (st) {                                        // one read of both counters
+        int64_t c[2];
+        int rc = read_counters(ctx, 2, c);
+        if (rc) return rc;
+        if (a->h_n_deactivated) *a->h_n_deactivated = a->seafloor_action == 2 ? c[0] : 0;
+        *h_undecided = c[1];
+        return OD_OK;
+    }
     return a->seafloor_action == 2 && a->h_n_deactivated ? read_counters(ctx, 1, a->h_n_deactivated) : OD_OK;
+}
+
+extern "C" int od_vertical_mixing(od_ctx* ctx, const od_mix_args* a) {
+    return mix_launch(ctx, a, nullptr, nullptr);
+}
+
+extern "C" int od_vertical_mixing_settle(od_ctx* ctx, const od_mix_args* a, int32_t* d_moving_out, int32_t* d_status_out,
+                                         int64_t* h_undecided) {
+    if (!h_undecided || (a && a->n > 0 && !d_moving_out)) return fail(ctx, OD_ERR_ARG, "od_vertical_mixing_settle: bad arguments");
+    *h_undecided = 0;
+    SettleParams st;
+    st.moving_out = d_moving_out;
+    st.status_out = a && a->seafloor_action == 2 ? d_status_out : nullptr;
+    st.undecided = nullptr;
+    return mix_launch(ctx, a, &st, h_undecided);
+}
+
+extern "C" int od_resuspend(od_ctx* ctx, int64_t n, const float* u, const float* v, float threshold, int32_t* moving, void* z,
+                            int32_t z_f64) {
+    if (!ctx || n < 0 || (n > 0 && (!u || !v || !moving || !z))) return fail(ctx, OD_ERR_ARG, "od_resuspend: bad arguments");
+    if (n == 0) return OD_OK;
+    CK(cudaSetDevice(ctx->device));
+    int64_t blocks = (n + 255) / 256;
+    if (blocks > (int64_t)ctx->sm_count * 8) blocks = (int64_t)ctx->sm_count * 8;
+    resuspend_kernel<<<(unsigned)blocks, 256, 0, ctx->stream>>>(n, u, v, threshold, moving, z, z_f64);
+    CK(cudaGetLastError());
+    ctx->launches++;
+    return OD_OK;
 }
 
 extern "C" int od_sort_by_cell(od_ctx* ctx, int group, int64_t n, const double* lon, const double* lat, const float* z,

@@ -199,8 +199,28 @@ OD_HD int nearest_level(const MixParams& p, const double* xs, const double* xy, 
     return zi < 0 ? 0 : (zi > nz - 1 ? nz - 1 : zi);
 }
 
-template <bool PROJ = false>
-OD_HD void mix_particle(const MixParams& p, int64_t i, const double* xs, const double* xy) {
+// SedimentDrift.bottom_interaction (sedimentdrift.py:108-116) inside the loop, kept apart from MixParams: with settling the input
+// moving / status are only read, and every element's values after the loop go to the outputs here.
+struct SettleParams {
+    int32_t* moving_out;         // [n]
+    int32_t* status_out;         // [n], or NULL when seafloor_action != 2
+    unsigned* undecided;         // elements whose settling depended on the others (see mix_particle)
+};
+
+OD_HD void count_one(unsigned* c) {
+#if defined(__CUDA_ARCH__)
+    atomicAdd(c, 1u);
+#else
+    *c += 1u;
+#endif
+}
+
+// SETTLE: after the sea floor, an element at or below Zmin that still moves settles (moving = 0 from there on).  The reference
+// calls bottom_interaction only in iterations where SOME element is below Zmin before the lift; an element that was below itself
+// decides that alone.  One that ends the iteration exactly at Zmin, moving, without having been below is left moving and counted
+// in *s->undecided: its result is only valid if no other element was below, which the caller cannot know from here.
+template <bool PROJ = false, bool SETTLE = false>
+OD_HD void mix_particle(const MixParams& p, int64_t i, const double* xs, const double* xy, const SettleParams* s = nullptr) {
     const GroupGeom& g = p.g;
     // the particle's diffusivity column (environment profile) is evaluated lazily, a window of levels at a time
     HorizW h;
@@ -226,6 +246,7 @@ OD_HD void mix_particle(const MixParams& p, int64_t i, const double* xs, const d
     const double r = 1.0 / 3;
     const unsigned id = p.ids ? (unsigned)p.ids[i] : (unsigned)i;
     double spare = 0.0;
+    bool settled = false, undecided = false;
     for (int it = 0; it < p.ntimes; ++it) {
         const bool surface = z == 0.0;
         const int zi = nearest_level(p, xs, xy, -z);
@@ -254,6 +275,7 @@ OD_HD void mix_particle(const MixParams& p, int64_t i, const double* xs, const d
         z = OD_DADD(z, OD_DMUL(OD_DMUL(w, p.dt_mix), mv));           // buoyancy
         if (!p.mix_at_surface && surface) z = 0.0;
         if (z > 0.0 && !p.skip_surface_stick) z = 0.0;                 // surface_stick
+        [[maybe_unused]] const bool below = z < zmin;            // before the lift
         if (p.seafloor_action && z < zmin) {                           // stick to the bottom
             z = zmin;
             if (p.seafloor_action == 2) {                              // deactivate_elements: moving = 0 from here on
@@ -261,9 +283,25 @@ OD_HD void mix_particle(const MixParams& p, int64_t i, const double* xs, const d
                 deactivated = true;
             }
         }
+        if constexpr (SETTLE) {
+            if (z <= zmin && mv == 1.0) {
+                if (below) {
+                    mv = 0.0;
+                    settled = true;
+                } else {
+                    undecided = true;
+                }
+            }
+        }
     }
     p.z_out[i] = z;
-    if (deactivated) {
+    if constexpr (SETTLE) {
+        const int32_t st = s->status_out ? p.status[i] : 0;
+        s->moving_out[i] = (settled || deactivated) ? 0 : (p.moving ? p.moving[i] : 1);
+        if (s->status_out) s->status_out[i] = (deactivated && st == 0) ? p.seafloor_code : st;
+        if (deactivated && p.counter) count_one(p.counter);
+        if (undecided) count_one(s->undecided);
+    } else if (deactivated) {
         if (p.status[i] == 0) p.status[i] = p.seafloor_code;
         p.moving_out[i] = 0;
 #if defined(__CUDA_ARCH__)
@@ -272,6 +310,17 @@ OD_HD void mix_particle(const MixParams& p, int64_t i, const double* xs, const d
         if (p.counter) *p.counter += 1u;
 #endif
     }
+}
+
+// SedimentDrift.resuspension (sedimentdrift.py:118-126) for one element: current_speed() squares the float32 environment components
+// and takes a float32 root (sqrtf is correctly rounded, as NumPy's), compared with the threshold as a float32 (NEP 50: a Python
+// float is weak); where it fires moving = 1 and z += 0.01 in z's own dtype.
+OD_HD void resuspend_one(int64_t i, const float* u, const float* v, float threshold, int32_t* moving, void* z, int z_f64) {
+    const float speed = sqrtf(OD_FADD(OD_FMUL(u[i], u[i]), OD_FMUL(v[i], v[i])));
+    if (!(speed > threshold && moving[i] == 0)) return;
+    moving[i] = 1;
+    if (z_f64) ((double*)z)[i] = OD_DADD(((double*)z)[i], 0.01);
+    else ((float*)z)[i] = OD_FADD(((float*)z)[i], 0.01f);
 }
 
 }  // namespace od

@@ -361,6 +361,59 @@ def default_engine(device=None):
     return _default[device]
 
 
+def _mix_args(eng, group, t, lon, lat, z_in, dt_mix, ntimes, moving=None, terminal_velocity=None, ids=None, rand=None, seed=0,
+              step_index=0, sea_floor=10000.0, mix_at_surface=False, pos_f32=False, model='environment', wind_speed=None, mld=50.0,
+              background=1.2e-5, k_const=0.0, seafloor_action=0, status=None, seafloor_code=0, iter0=0, skip_surface_stick=False):
+    """(od_mix_args, float64 z_out tensor, deactivation count) of Engine.vertical_mixing and vertical_mixing_settle"""
+    torch = eng.torch
+    n = lon.numel()
+    z_out = eng.empty(n, torch.float64)
+    a = MixArgs()
+    a.ntimes = int(ntimes)
+    a.model = eng.MIX_MODELS[model]
+    if a.model == _lib.OD_MIX_ENVIRONMENT:
+        a.group_k = group.gid
+        a.t_k, _ = group.sample(t)
+    else:
+        a.group_k = -1
+        if hasattr(mld, 'data_ptr'):
+            assert mld.dtype == torch.float32
+            a.d_mld = mld.data_ptr()
+            mld_max = float(eng.minmax(mld)[1])
+        else:
+            a.mld_const = float(np.float32(mld))
+            mld_max = float(np.float32(mld))
+        a.nlev = len(np.arange(0, np.float32(mld_max) + 2))          # mixing_z = -np.arange(0, MLD.max() + 2)
+        if wind_speed is not None:
+            assert wind_speed.dtype == torch.float32
+            a.d_wind_speed = wind_speed.data_ptr()
+        a.background, a.k_const = float(background), float(k_const)
+    a.n = n
+    a.d_lon, a.d_lat = lon.data_ptr(), lat.data_ptr()
+    a.d_z_in, a.z_in_f64 = z_in.data_ptr(), 1 if z_in.dtype == torch.float64 else 0
+    a.d_z_out = z_out.data_ptr()
+    a.d_moving = moving.data_ptr() if moving is not None else None
+    if terminal_velocity is not None:
+        a.d_terminal_velocity = terminal_velocity.data_ptr()
+        a.tv_f64 = 1 if terminal_velocity.dtype == torch.float64 else 0
+    a.d_ids = ids.data_ptr() if ids is not None else None
+    a.d_rand = rand.data_ptr() if rand is not None else None
+    if hasattr(sea_floor, 'data_ptr'):
+        a.d_sea_floor = sea_floor.data_ptr()
+    else:
+        a.sea_floor_const = float(sea_floor)
+    a.dt_mix, a.seed, a.step_index = float(dt_mix), int(seed), int(step_index)
+    a.mix_at_surface, a.pos_f32 = (1 if mix_at_surface else 0), (1 if pos_f32 else 0)
+    a.iter0, a.skip_surface_stick = int(iter0), 1 if skip_surface_stick else 0
+    a.seafloor_action = int(seafloor_action)          # 'stick to bottom' with a sea-floor reader: 1 lift, 2 deactivate
+    nd = C.c_int64(0)
+    if a.seafloor_action == 2:
+        assert status is not None and moving is not None and status.dtype == torch.int32
+        a.d_status, a.d_moving_out, a.seafloor_code = status.data_ptr(), moving.data_ptr(), int(seafloor_code)
+        a.h_n_deactivated = C.pointer(nd)
+    return a, z_out, nd
+
+
 class Engine:
     def __init__(self, device=0):
         import torch
@@ -960,63 +1013,38 @@ class Engine:
     MIX_MODELS = {'environment': _lib.OD_MIX_ENVIRONMENT, 'windspeed_Large1994': _lib.OD_MIX_LARGE1994,
                   'windspeed_Sundby1983': _lib.OD_MIX_SUNDBY1983, 'constant': _lib.OD_MIX_CONSTANT}
 
-    def vertical_mixing(self, group, t, lon, lat, z_in, dt_mix, ntimes, moving=None, terminal_velocity=None, ids=None,
-                        rand=None, seed=0, step_index=0, sea_floor=10000.0, mix_at_surface=False, pos_f32=False,
-                        model='environment', wind_speed=None, mld=50.0, background=1.2e-5, k_const=0.0, seafloor_action=0,
-                        status=None, seafloor_code=0, iter0=0, skip_surface_stick=False):
+    def vertical_mixing(self, group, t, lon, lat, z_in, dt_mix, ntimes, **kw):
         """OceanDrift.vertical_mixing on device tensors; returns the new depth (float64 tensor).
         model 'environment' takes the diffusivity column from `group`; 'windspeed_Large1994' / 'windspeed_Sundby1983' /
         'constant' build it analytically on 1 m levels from wind_speed (float32 tensor) and the mixed layer depth mld
         (float32 tensor or scalar), as oceandrift.py:429-453 does when no ocean-model diffusivity is available."""
-        torch = self.torch
-        n = lon.numel()
-        z_out = self.empty(n, torch.float64)
-        a = MixArgs()
-        a.ntimes = int(ntimes)
-        a.model = self.MIX_MODELS[model]
-        if a.model == _lib.OD_MIX_ENVIRONMENT:
-            a.group_k = group.gid
-            a.t_k, _ = group.sample(t)
-        else:
-            a.group_k = -1
-            if hasattr(mld, 'data_ptr'):
-                assert mld.dtype == torch.float32
-                a.d_mld = mld.data_ptr()
-                mld_max = float(self.minmax(mld)[1])
-            else:
-                a.mld_const = float(np.float32(mld))
-                mld_max = float(np.float32(mld))
-            a.nlev = len(np.arange(0, np.float32(mld_max) + 2))          # mixing_z = -np.arange(0, MLD.max() + 2)
-            if wind_speed is not None:
-                assert wind_speed.dtype == torch.float32
-                a.d_wind_speed = wind_speed.data_ptr()
-            a.background, a.k_const = float(background), float(k_const)
-        a.n = n
-        a.d_lon, a.d_lat = lon.data_ptr(), lat.data_ptr()
-        a.d_z_in, a.z_in_f64 = z_in.data_ptr(), 1 if z_in.dtype == torch.float64 else 0
-        a.d_z_out = z_out.data_ptr()
-        a.d_moving = moving.data_ptr() if moving is not None else None
-        if terminal_velocity is not None:
-            a.d_terminal_velocity = terminal_velocity.data_ptr()
-            a.tv_f64 = 1 if terminal_velocity.dtype == torch.float64 else 0
-        a.d_ids = ids.data_ptr() if ids is not None else None
-        a.d_rand = rand.data_ptr() if rand is not None else None
-        if hasattr(sea_floor, 'data_ptr'):
-            a.d_sea_floor = sea_floor.data_ptr()
-        else:
-            a.sea_floor_const = float(sea_floor)
-        a.dt_mix, a.seed, a.step_index = float(dt_mix), int(seed), int(step_index)
-        a.mix_at_surface, a.pos_f32 = (1 if mix_at_surface else 0), (1 if pos_f32 else 0)
-        a.iter0, a.skip_surface_stick = int(iter0), 1 if skip_surface_stick else 0
-        a.seafloor_action = int(seafloor_action)          # 'stick to bottom' with a sea-floor reader: 1 lift, 2 deactivate
-        nd = C.c_int64(0)
-        if a.seafloor_action == 2:
-            assert status is not None and moving is not None and status.dtype == torch.int32
-            a.d_status, a.d_moving_out, a.seafloor_code = status.data_ptr(), moving.data_ptr(), int(seafloor_code)
-            a.h_n_deactivated = C.pointer(nd)
+        a, z_out, nd = _mix_args(self, group, t, lon, lat, z_in, dt_mix, ntimes, **kw)
         self._check(self.lib.od_vertical_mixing(self.ctx, C.byref(a)))
         self.last_mix_deactivated = int(nd.value)
         return z_out
+
+    def vertical_mixing_settle(self, group, t, lon, lat, z_in, dt_mix, ntimes, **kw):
+        """vertical_mixing with SedimentDrift.bottom_interaction in every inner iteration (od_vertical_mixing_settle).  moving and
+        status are only read; returns (z_out float64, moving_out int32, status_out int32 or None, undecided count).  A non-zero
+        count: some element's settling depended on the other elements, and the result is not the reference's."""
+        a, z_out, nd = _mix_args(self, group, t, lon, lat, z_in, dt_mix, ntimes, **kw)
+        torch = self.torch
+        n = lon.numel()
+        moving_out = self.empty(n, torch.int32)
+        status_out = self.empty(n, torch.int32) if a.seafloor_action == 2 else None
+        und = C.c_int64(0)
+        self._check(self.lib.od_vertical_mixing_settle(self.ctx, C.byref(a), _ptr(moving_out), _ptr(status_out), C.byref(und)))
+        self.last_mix_deactivated = int(nd.value)
+        return z_out, moving_out, status_out, int(und.value)
+
+    def resuspend(self, u, v, threshold, moving, z):
+        """SedimentDrift.resuspension in place: moving = 1 and z += 0.01 where float32 sqrt(u*u + v*v) > float32(threshold) and
+        moving == 0.  u, v: float32; moving: int32; z: float32 or float64."""
+        torch = self.torch
+        assert u.dtype == v.dtype == torch.float32 and moving.dtype == torch.int32 and z.dtype in (torch.float32, torch.float64)
+        assert u.numel() == v.numel() == moving.numel() == z.numel()
+        self._check(self.lib.od_resuspend(self.ctx, z.numel(), _ptr(u), _ptr(v), float(np.float32(threshold)), _ptr(moving), _ptr(z),
+                                          1 if z.dtype == torch.float64 else 0))
 
     # -- particle exchange of the spatial-tile mode (od_pack_by_owner / od_unpack_records) --------------------------------------
     def pack_by_owner(self, lon, bounds, columns, want_perm=False):

@@ -138,6 +138,11 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
     ElementType = LagrangianArray
     required_variables = {}
     status_categories = ['active']
+    # the reference's general:coastline_action default (against the GSHHG mask) and what it does, named by the warning of
+    # _setup_coastline
+    _coast_reference_default = ('stranding', 'strand elements on that mask')
+    # a model whose decisions the reference takes over the whole element array names itself here: refused in distributed runs
+    _distributed_refusal = None
 
     def __init__(self, seed=0, loglevel=None, logfile=None, engine=None, **kwargs):
         Configurable.__init__(self)
@@ -506,9 +511,10 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
             # The reference's default is 'stranding' (against the GSHHG landmask, which is not on this path); the default here is
             # 'none'.  A script that adds a land_binary_mask reader and leaves the action alone would strand under the reference.
             self._coast_default_warned = True
+            ref_default, what = self._coast_reference_default
             logger.warning("a reader provides land_binary_mask but general:coastline_action is 'none' (the default of the GPU classes; the "
-                           "reference's default is 'stranding'): set general:coastline_action = 'stranding' and "
-                           "general:coastline_approximation_precision = None to strand elements on that mask")
+                           "reference's default is '%s'): set general:coastline_action = '%s' and "
+                           "general:coastline_approximation_precision = None to %s" % (ref_default, ref_default, what))
         if action == 'none' or 'land_binary_mask' not in self.required_variables:
             return
         if self.env.constant('land_binary_mask') is not None and not self.env.priority_list.get('land_binary_mask'):
@@ -1089,6 +1095,8 @@ class OpenDriftSimulation(PhysicsMethods, Configurable):
             # the reference decides whether to replace the Stokes drift and Hs from their maxima over the whole element array;
             # a shard sees only its own elements
             raise NotImplementedError('drift:use_tabularised_stokes_drift = True is not on the distributed GPU path')
+        if self._dist is not None and self._distributed_refusal:
+            raise NotImplementedError('%s is not on the distributed GPU path' % self._distributed_refusal)
         self.shard = None
         if self._dist is not None and self.get_config('gpu:shard') == 'index':
             n_all = int(self.num_elements_total())

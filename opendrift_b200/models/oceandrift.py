@@ -267,6 +267,21 @@ class OceanDrift(OpenDriftSimulation):
 
     def _mix(self, lon0, lat0, z_in, pos_f32):
         """Run the mixing kernel from start-of-step positions; returns the new float64 depth tensor."""
+        eng = self.engine
+        m = self._mix_setup(lon0, lat0, z_in, pos_f32)
+        hooks = self._overridden_mixing_hooks()
+        if not hooks:
+            # the whole inner loop in one launch
+            z_out = eng.vertical_mixing(m['g'], self.time, lon0, lat0, z_in, m['dt_mix'], m['ntimes'], terminal_velocity=m['tv'],
+                                        rand=self._mix_draws(m), seafloor_action=m['action'], status=m['status'],
+                                        seafloor_code=m['code'], **m['common'])
+            if m['action'] == 2 and getattr(eng, 'last_mix_deactivated', 0):
+                self._seafloor_deactivated()
+            return z_out
+        return self._mix_iterations(m, hooks)
+
+    def _mix_setup(self, lon0, lat0, z_in, pos_f32):
+        """The arguments of the mixing launches of one time step."""
         eng, el, torch = self.engine, self.elements, self.engine.torch
         g, model, dt_mix, ntimes, floor = self._mixing_inputs()
         # Zmin = -1.*(sea_floor_depth + sea_surface_height) (:420): the kernel negates the float32 column it is handed
@@ -305,32 +320,44 @@ class OceanDrift(OpenDriftSimulation):
                 moving = el.dev('moving', torch.int32)
         common = dict(moving=moving, ids=ids, seed=getattr(self, '_seed', 0), step_index=self.steps_calculation, sea_floor=floor,
                       mix_at_surface=self.get_config('drift:vertical_mixing_at_surface'), pos_f32=pos_f32, **kw)
-        hooks = self._overridden_mixing_hooks()
-        if not hooks:
-            # the whole inner loop in one launch
-            rand = None
-            if self.get_config('gpu:rng') == 'numpy':          # the reference's draws, in its order (:524)
-                rand = eng.to_device(np.ascontiguousarray(np.stack([np.random.random(n) for _ in range(ntimes)])))
-            z_out = eng.vertical_mixing(g, self.time, lon0, lat0, z_in, dt_mix, ntimes, terminal_velocity=tv, rand=rand,
-                                        seafloor_action=action, status=status, seafloor_code=code, **common)
-            if action == 2 and getattr(eng, 'last_mix_deactivated', 0):
-                if 'seafloor' not in self.status_categories:
-                    self.status_categories.append('seafloor')
-                self._maybe_deactivated = True
-            return z_out
-        # A subclass overrides a per-iteration hook: one launch per inner iteration, the hooks in between, in the reference's
-        # order (:515-564): [update_terminal_velocity] random walk + reflections + buoyancy [surface_stick] [surface_wave_mixing]
-        # sea floor [bottom_interaction].  The draws of the legacy generator are made iteration by iteration, as the reference does
-        # (a hook may draw too); the device generator continues its per-step stream (iter0).
+        return dict(g=g, dt_mix=dt_mix, ntimes=ntimes, floor=floor, n=n, tv=tv, action=action, code=code, status=status,
+                    common=common, lon0=lon0, lat0=lat0, z_in=z_in)
+
+    def _mix_draws(self, m):
+        """[ntimes][n] draws of the legacy generator for a launch of the whole inner loop (the reference's, in its order, :524),
+        or None with gpu:rng = philox."""
+        if self.get_config('gpu:rng') != 'numpy':
+            return None
+        return self.engine.to_device(np.ascontiguousarray(np.stack([np.random.random(m['n']) for _ in range(m['ntimes'])])))
+
+    def _seafloor_deactivated(self):
+        if 'seafloor' not in self.status_categories:
+            self.status_categories.append('seafloor')
+        self._maybe_deactivated = True
+
+    def _mix_iterations(self, m, hooks, rows=None):
+        """A subclass overrides a per-iteration hook: one launch per inner iteration, the hooks in between, in the reference's
+        order (:515-564): [update_terminal_velocity] random walk + reflections + buoyancy [surface_stick] [surface_wave_mixing]
+        sea floor [bottom_interaction].  The draws of the legacy generator are made iteration by iteration, as the reference does
+        (a hook may draw too), unless rows holds this step's draws already made; the device generator continues its per-step
+        stream (iter0)."""
+        eng, el, torch = self.engine, self.elements, self.engine.torch
+        g, dt_mix, common, tv, action, code, floor = m['g'], m['dt_mix'], dict(m['common']), m['tv'], m['action'], m['code'], m['floor']
+        lon0, lat0, n = m['lon0'], m['lat0'], m['n']
         self.prepare_vertical_mixing()
-        z = z_in
+        z = m['z_in']
         numpy_rng = self.get_config('gpu:rng') == 'numpy'
-        for it in range(ntimes):
+        for it in range(m['ntimes']):
             if 'update_terminal_velocity' in hooks:
                 el.set_dev('z', z)
                 self.update_terminal_velocity(Tprofiles=None, Sprofiles=None, z_index=None)
                 tv = el.dev('terminal_velocity')
-            r = eng.to_device(np.ascontiguousarray(np.random.random(n)[None])) if numpy_rng else None
+            if rows is not None:
+                r = rows[it:it + 1]
+            else:
+                r = eng.to_device(np.ascontiguousarray(np.random.random(n)[None])) if numpy_rng else None
+            moving = el.dev('moving')              # as a hook (bottom_interaction) may have left it
+            common['moving'] = moving if moving.dtype == torch.int32 else moving.to(torch.int32)
             z = eng.vertical_mixing(g, self.time, lon0, lat0, z, dt_mix, 1, terminal_velocity=tv, rand=r, iter0=it,
                                     skip_surface_stick='surface_stick' in hooks, **common)
             el.set_dev('z', z)
@@ -362,9 +389,7 @@ class OceanDrift(OpenDriftSimulation):
                                    moving=el.dev('moving', torch.int32), seafloor_code=code if action == 2 else 0, count=action == 2)
         el.set_dev('z', z)
         if nd:
-            if 'seafloor' not in self.status_categories:
-                self.status_categories.append('seafloor')
-            self._maybe_deactivated = True
+            self._seafloor_deactivated()
 
     def vertical_mixing(self, store_depths=False):
         """Helper for subclasses that override update(): uses the start-of-step positions saved by the run loop."""
