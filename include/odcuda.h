@@ -467,6 +467,22 @@ int od_vertical_mixing_settle(od_ctx* ctx, const od_mix_args* a, int32_t* d_movi
  * moving == 0, moving = 1 and z += 0.01 in z's dtype (float64 when z_f64, else float32).  u, v: the step's float32 current. */
 int od_resuspend(od_ctx* ctx, int64_t n, const float* d_u, const float* d_v, float threshold, int32_t* d_moving, void* d_z, int32_t z_f64);
 
+/* ---- ShipDrift ---------------------------------------------------------------------------------
+ * ShipDrift.update (models/shipdrift.py:216-343) for n ships in one launch, from the float32 start-of-step environment: the current
+ * move, then the move with the velocity of the wind / wave / form-drag force balance, then the stranding flag.
+ *   d_el: the six float32 element arrays length, height, draft, beam, wind_drag_coeff, water_drag_coeff (a host array of 6 device
+ *         pointers); d_orientation: uint8.
+ *   d_env: float32 x_sea_water_velocity, y_sea_water_velocity, x_wind, y_wind, Hs, period, Stokes x, Stokes y, land_binary_mask
+ *         (a host array of 9 device pointers; Stokes NULL: the wave direction is the wind's; mask NULL: no stranding).
+ *   hs_wind: Hs = 0.0246 ws^2, written into the Hs array; tm_wind: the period from the wind (float64 arithmetic), written into the
+ *   period array as float32; tm_fill_on: period values of exactly 0 are replaced by tm_fill.
+ *   d_wtab / d_wbox: the wforce.dat table and its Delaunay tetrahedra per grid box (layout in csrc/od_ship.cuh).
+ *   Where land_binary_mask == 1: status = strand_code (when 0) and moving = 0; *h_stranded = 1 if that happened (synchronises). */
+int od_ship_step(od_ctx* ctx, int64_t n, double* d_lon, double* d_lat, int32_t* d_moving, int32_t* d_status, const float* const* d_el,
+                 const uint8_t* d_orientation, float* const* d_env, const double* d_wtab, const int32_t* d_wbox, int32_t nomega,
+                 int32_t nbeam, int32_t ndraft, int32_t hs_wind, int32_t tm_wind, int32_t tm_fill_on, float tm_fill, int32_t strand_code,
+                 double dt, int32_t* h_stranded);
+
 /* ---- analytical readers on a projected plane ---------------------------------------------------------
  * BASELINE configs[0]: opendrift/readers/reader_double_gyre.py (a ContinuousReader, basereader/continuous.py:9-48) on the
  * spherical stereographic plane its constructor asks pyproj for (reader_double_gyre.py:27-31).  The reader chain of

@@ -204,6 +204,8 @@ SYMBOLS = {
     'od_vertical_mixing': (C.c_int, [_P, C.POINTER(MixArgs)]),
     'od_vertical_mixing_settle': (C.c_int, [_P, C.POINTER(MixArgs), _P, _P, C.POINTER(C.c_int64)]),
     'od_resuspend': (C.c_int, [_P, C.c_int64, _P, _P, C.c_float, _P, _P, C.c_int32]),
+    'od_ship_step': (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                               C.c_int32, C.c_float, C.c_int32, C.c_double, C.POINTER(C.c_int32)]),
     'od_vertical_buoyancy': (C.c_int, [_P, C.POINTER(BuoyancyArgs)]),
     'od_bookkeeping': (C.c_int, [_P, C.POINTER(BookkeepArgs)]),
     'od_coastline': (C.c_int, [_P, C.POINTER(CoastArgs)]),

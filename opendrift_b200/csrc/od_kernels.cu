@@ -20,6 +20,7 @@
 #include "od_mix.cuh"
 #include "od_stokes.cuh"
 #include "od_leeway.cuh"
+#include "od_ship.cuh"
 #include "od_analytic.cuh"
 #include "od_history.cuh"
 #include "od_bookkeep.cuh"
@@ -700,6 +701,12 @@ __global__ void __launch_bounds__(256) resuspend_kernel(int64_t n, const float* 
                                                         float threshold, int32_t* __restrict__ moving, void* __restrict__ z, int32_t z_f64) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
         resuspend_one(i, u, v, threshold, moving, z, z_f64);
+}
+
+// ---- ShipDrift -----------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) ship_kernel(const ShipParams p) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += (int64_t)gridDim.x * blockDim.x)
+        ship_particle(p, i);
 }
 
 // ---- Leeway -------------------------------------------------------------------------------------------
@@ -1821,6 +1828,49 @@ extern "C" int od_resuspend(od_ctx* ctx, int64_t n, const float* u, const float*
     resuspend_kernel<<<(unsigned)blocks, 256, 0, ctx->stream>>>(n, u, v, threshold, moving, z, z_f64);
     CK(cudaGetLastError());
     ctx->launches++;
+    return OD_OK;
+}
+
+extern "C" int od_ship_step(od_ctx* ctx, int64_t n, double* lon, double* lat, int32_t* moving, int32_t* status, const float* const* el,
+                            const uint8_t* orientation, float* const* env, const double* wtab, const int32_t* wbox, int32_t nomega,
+                            int32_t nbeam, int32_t ndraft, int32_t hs_wind, int32_t tm_wind, int32_t tm_fill_on, float tm_fill,
+                            int32_t strand_code, double dt, int32_t* h_stranded) {
+    if (!ctx || n < 0 || !el || !env || !h_stranded || nomega < 2 || nbeam < 2 || ndraft < 2)
+        return fail(ctx, OD_ERR_ARG, "od_ship_step: bad arguments");
+    *h_stranded = 0;
+    if (n == 0) return OD_OK;
+    if (!lon || !lat || !orientation || !wtab || !wbox || !env[0] || !env[1] || !env[2] || !env[3] || !env[4] || !env[5] ||
+        (!env[6]) != (!env[7]) || (env[8] && !status))
+        return fail(ctx, OD_ERR_ARG, "od_ship_step: bad arguments");
+    for (int k = 0; k < 6; ++k)
+        if (!el[k]) return fail(ctx, OD_ERR_ARG, "od_ship_step: null element array");
+    CK(cudaSetDevice(ctx->device));
+    ShipParams p;
+    memset(&p, 0, sizeof(p));
+    p.n = n; p.lon = lon; p.lat = lat; p.moving = moving; p.status = status;
+    p.length = el[0]; p.height = el[1]; p.draft = el[2]; p.beam = el[3]; p.cf = el[4]; p.cd = el[5];
+    p.orientation = orientation;
+    p.cu = env[0]; p.cv = env[1]; p.xw = env[2]; p.yw = env[3]; p.hs = env[4]; p.tm = env[5]; p.sx = env[6]; p.sy = env[7];
+    p.mask = env[8];
+    p.wtab = wtab; p.wbox = wbox; p.nomega = nomega; p.nbeam = nbeam; p.ndraft = ndraft;
+    p.hs_wind = hs_wind; p.tm_wind = tm_wind; p.tm_fill_on = tm_fill_on; p.tm_fill = tm_fill; p.strand_code = strand_code;
+    p.dt = dt;
+    if (p.mask) {
+        if (!ctx->d_red) CK(cudaMalloc(&ctx->d_red, 2 * sizeof(unsigned)));
+        CK(cudaMemsetAsync(ctx->d_red, 0, sizeof(unsigned), ctx->stream));
+        p.stranded = ctx->d_red;
+    }
+    int64_t blocks = (n + 255) / 256;
+    if (blocks > (int64_t)ctx->sm_count * 8) blocks = (int64_t)ctx->sm_count * 8;
+    ship_kernel<<<(unsigned)blocks, 256, 0, ctx->stream>>>(p);
+    CK(cudaGetLastError());
+    ctx->launches++;
+    if (p.mask) {
+        unsigned flag = 0;
+        CK(cudaMemcpyAsync(&flag, ctx->d_red, sizeof(flag), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        *h_stranded = flag ? 1 : 0;
+    }
     return OD_OK;
 }
 

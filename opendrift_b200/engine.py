@@ -83,6 +83,12 @@ def _ptr(t):
     return C.c_void_p(t.data_ptr())
 
 
+# od_ship_step's element and environment arrays, in the order of its pointer tables
+SHIP_ELEMENTS = ('length', 'height', 'draft', 'beam', 'wind_drag_coeff', 'water_drag_coeff')
+SHIP_ENV = ('x_sea_water_velocity', 'y_sea_water_velocity', 'x_wind', 'y_wind', 'hs', 'period', 'stokes_x', 'stokes_y',
+            'land_binary_mask')
+
+
 def grid_geometry(lon, lat):
     """What the sampler needs to know about a regular float32 lon/lat grid, following the reference:
     * Linear2DInterpolator (interpolators.py:110-111): xi = (x - xg[0]) / (xg[-1] - xg[0]) * (nx - 1), float32 end points and
@@ -1045,6 +1051,34 @@ class Engine:
         assert u.numel() == v.numel() == moving.numel() == z.numel()
         self._check(self.lib.od_resuspend(self.ctx, z.numel(), _ptr(u), _ptr(v), float(np.float32(threshold)), _ptr(moving), _ptr(z),
                                           1 if z.dtype == torch.float64 else 0))
+
+    def ship_step(self, lon, lat, moving, status, el, orientation, env, table, dt, hs_wind=False, tm_wind=False, tm_fill=None,
+                  strand_code=0):
+        """ShipDrift.update in one launch (od_ship_step): the current move, then the move with the force-balance velocity, then the
+        stranding flag.  el: dict of the float32 tensors SHIP_ELEMENTS; orientation: uint8; env: dict of the float32 tensors SHIP_ENV
+        (stokes_x / stokes_y / land_binary_mask may be None; hs and period are written when hs_wind / tm_wind); table: (wtab float64,
+        wbox int32, (nomega, nbeam, ndraft)) on the device.  tm_fill: the value that replaces a period of exactly 0, or None.
+        Returns True when a ship stranded (status = strand_code, moving = 0)."""
+        torch = self.torch
+        n = lon.numel()
+        assert lon.dtype == lat.dtype == torch.float64 and orientation.dtype == torch.uint8
+        assert moving is None or moving.dtype == torch.int32
+        assert status is None or status.dtype == torch.int32
+        els = [el[k] for k in SHIP_ELEMENTS]
+        envs = [env.get(k) for k in SHIP_ENV]
+        for t in els + [e for e in envs if e is not None]:
+            assert t.dtype == torch.float32 and t.numel() == n and t.is_contiguous()
+        wtab, wbox, (nomega, nbeam, ndraft) = table
+        assert wtab.dtype == torch.float64 and wbox.dtype == torch.int32
+        el_p = (C.c_void_p * 6)(*[t.data_ptr() for t in els])
+        env_p = (C.c_void_p * 9)(*[None if t is None else t.data_ptr() for t in envs])
+        stranded = C.c_int32()
+        self._check(self.lib.od_ship_step(self.ctx, n, _ptr(lon), _ptr(lat), _ptr(moving), _ptr(status), el_p, _ptr(orientation),
+                                          env_p, _ptr(wtab), _ptr(wbox), nomega, nbeam, ndraft, int(bool(hs_wind)),
+                                          int(bool(tm_wind)), 0 if tm_fill is None else 1,
+                                          float(np.float32(0 if tm_fill is None else tm_fill)), int(strand_code), float(dt),
+                                          C.byref(stranded)))
+        return bool(stranded.value)
 
     # -- particle exchange of the spatial-tile mode (od_pack_by_owner / od_unpack_records) --------------------------------------
     def pack_by_owner(self, lon, bounds, columns, want_perm=False):

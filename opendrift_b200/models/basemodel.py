@@ -54,6 +54,11 @@ class EnvironmentView:
             self._t[name] = engine.to_device(np.ascontiguousarray(self._h.pop(name)))
         return self._t[name]
 
+    def set_dev(self, name, tensor):
+        """Replace a variable by a device tensor (a model that computes it on the device writes it back this way)."""
+        self._h.pop(name, None)
+        self._t[name] = tensor
+
     def __contains__(self, name):
         return name in self._t or name in self._h
 
