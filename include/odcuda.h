@@ -483,6 +483,24 @@ int od_ship_step(od_ctx* ctx, int64_t n, double* d_lon, double* d_lat, int32_t* 
                  int32_t nbeam, int32_t ndraft, int32_t hs_wind, int32_t tm_wind, int32_t tm_fill_on, float tm_fill, int32_t strand_code,
                  double dt, int32_t* h_stranded);
 
+/* ---- PlastDrift ---------------------------------------------------------------------------------
+ * PlastDrift.update after the current move (models/plastdrift.py:80-107) for n elements in one launch, each element in turn:
+ *   (a) with d_z_out: z = -(double(K / tv) * E) written to d_z_out (float64), for every element whatever `moving`.
+ *       K: float32 ocean_vertical_diffusivity; tv: terminal_velocity, float32 or float64 (tv_f64), the quotient in tv's dtype.
+ *       E: d_rand (float64 standard exponential draws) or, with d_rand NULL, -log(1 - u) with u from Philox keyed by
+ *       (seed, d_ids[i], step_index, a tag of its own).
+ *       *h_negative = 1 if some scale is negative and not NaN (synchronises); without d_z_out the depth is d_z_in (z_f64).
+ *   (b) with d_stokes (a host array of 11 device pointers: Stokes x, y, Hs, x_wind, y_wind, then the six windsea_swell arrays,
+ *       as in od_stokes_args): the Stokes move at the element's depth (hs_mode, profile as in od_stokes_args).
+ *   (c) with d_wdf (wind_drift_factor, float32 or float64: wdf_f64): the wind move at the element's depth, with
+ *       drift:wind_drift_depth = wind_drift_depth.
+ * (b) and (c) move only where d_moving != 0 (NULL: everywhere). */
+int od_plast_step(od_ctx* ctx, int64_t n, double* d_lon, double* d_lat, const int32_t* d_moving, const void* d_z_in, int32_t z_f64,
+                  double* d_z_out, const float* d_k, const void* d_tv, int32_t tv_f64, const double* d_rand, const int32_t* d_ids,
+                  unsigned long long seed, int32_t step_index, const float* const* d_stokes, int32_t hs_mode, int32_t profile,
+                  const float* d_xwind, const float* d_ywind, const void* d_wdf, int32_t wdf_f64, double wind_drift_depth, double dt,
+                  int32_t* h_negative);
+
 /* ---- analytical readers on a projected plane ---------------------------------------------------------
  * BASELINE configs[0]: opendrift/readers/reader_double_gyre.py (a ContinuousReader, basereader/continuous.py:9-48) on the
  * spherical stereographic plane its constructor asks pyproj for (reader_double_gyre.py:27-31).  The reader chain of

@@ -206,6 +206,8 @@ SYMBOLS = {
     'od_resuspend': (C.c_int, [_P, C.c_int64, _P, _P, C.c_float, _P, _P, C.c_int32]),
     'od_ship_step': (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, _P, _P, _P, _P, _P, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                C.c_int32, C.c_float, C.c_int32, C.c_double, C.POINTER(C.c_int32)]),
+    'od_plast_step': (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, C.c_int32, _P, _P, _P, C.c_int32, _P, _P, C.c_uint64, C.c_int32, _P, C.c_int32,
+                                C.c_int32, _P, _P, _P, C.c_int32, C.c_double, C.c_double, C.POINTER(C.c_int32)]),
     'od_vertical_buoyancy': (C.c_int, [_P, C.POINTER(BuoyancyArgs)]),
     'od_bookkeeping': (C.c_int, [_P, C.POINTER(BookkeepArgs)]),
     'od_coastline': (C.c_int, [_P, C.POINTER(CoastArgs)]),

@@ -21,6 +21,7 @@
 #include "od_stokes.cuh"
 #include "od_leeway.cuh"
 #include "od_ship.cuh"
+#include "od_plast.cuh"
 #include "od_analytic.cuh"
 #include "od_history.cuh"
 #include "od_bookkeep.cuh"
@@ -707,6 +708,12 @@ __global__ void __launch_bounds__(256) resuspend_kernel(int64_t n, const float* 
 __global__ void __launch_bounds__(256) ship_kernel(const ShipParams p) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += (int64_t)gridDim.x * blockDim.x)
         ship_particle(p, i);
+}
+
+// ---- PlastDrift ----------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(OD_BLOCK) plast_kernel(const PlastParams p) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += (int64_t)gridDim.x * blockDim.x)
+        plast_particle(p, i);
 }
 
 // ---- Leeway -------------------------------------------------------------------------------------------
@@ -1870,6 +1877,58 @@ extern "C" int od_ship_step(od_ctx* ctx, int64_t n, double* lon, double* lat, in
         CK(cudaMemcpyAsync(&flag, ctx->d_red, sizeof(flag), cudaMemcpyDeviceToHost, ctx->stream));
         CK(cudaStreamSynchronize(ctx->stream));
         *h_stranded = flag ? 1 : 0;
+    }
+    return OD_OK;
+}
+
+extern "C" int od_plast_step(od_ctx* ctx, int64_t n, double* lon, double* lat, const int32_t* moving, const void* z_in, int32_t z_f64,
+                             double* z_out, const float* k, const void* tv, int32_t tv_f64, const double* rand, const int32_t* ids,
+                             unsigned long long seed, int32_t step_index, const float* const* stokes, int32_t hs_mode, int32_t profile,
+                             const float* xwind, const float* ywind, const void* wdf, int32_t wdf_f64, double wind_drift_depth, double dt,
+                             int32_t* h_negative) {
+    if (!ctx || n < 0 || !h_negative) return fail(ctx, OD_ERR_ARG, "od_plast_step: bad arguments");
+    *h_negative = 0;
+    if (stokes && (hs_mode < 0 || hs_mode > 2 || profile < 0 || profile > 3))
+        return fail(ctx, OD_ERR_ARG, "od_plast_step: bad Stokes mode");
+    if (n == 0) return OD_OK;
+    if (!lon || !lat || (!z_out && !z_in) || (z_out && (!k || !tv)) || (wdf && (!xwind || !ywind)) ||
+        (stokes && (!stokes[0] || !stokes[1] || (hs_mode == 0 && profile != 3 && !stokes[2]))))
+        return fail(ctx, OD_ERR_ARG, "od_plast_step: bad arguments");
+    if (stokes && profile == 3)
+        for (int j = 5; j < 11; ++j)
+            if (!stokes[j]) return fail(ctx, OD_ERR_ARG, "od_plast_step: the windsea_swell profile needs the six swell / wind-sea arrays");
+    CK(cudaSetDevice(ctx->device));
+    PlastParams p;
+    memset(&p, 0, sizeof(p));
+    p.n = n; p.lon = lon; p.lat = lat; p.moving = moving; p.z_in = z_in; p.z_f64 = z_f64; p.z_out = z_out;
+    p.k = k; p.tv = tv; p.tv_f64 = tv_f64; p.rand = rand; p.ids = ids; p.seed = seed; p.step_index = step_index;
+    if (stokes) {
+        p.stokes_on = 1;
+        p.st.us = stokes[0]; p.st.vs = stokes[1]; p.st.hs = stokes[2]; p.st.xwind = stokes[3]; p.st.ywind = stokes[4];
+        p.st.sw_dir = stokes[5]; p.st.sw_period = stokes[6]; p.st.sw_hs = stokes[7];
+        p.st.ws_dir = stokes[8]; p.st.ws_period = stokes[9]; p.st.ws_hs = stokes[10];
+        p.st.hs_mode = hs_mode; p.st.profile = profile; p.st.factor = 1.0;
+    }
+    if (wdf) {
+        p.wind_on = 1;
+        p.xwind = xwind; p.ywind = ywind; p.wdf = wdf; p.wdf_f64 = wdf_f64; p.wdd = fabs(wind_drift_depth);
+    }
+    p.dt = dt;
+    if (z_out) {
+        if (!ctx->d_red) CK(cudaMalloc(&ctx->d_red, 2 * sizeof(unsigned)));
+        CK(cudaMemsetAsync(ctx->d_red, 0, sizeof(unsigned), ctx->stream));
+        p.negative = ctx->d_red;
+    }
+    int64_t blocks = (n + OD_BLOCK - 1) / OD_BLOCK;
+    if (blocks > (int64_t)ctx->sm_count * 8) blocks = (int64_t)ctx->sm_count * 8;
+    plast_kernel<<<(unsigned)blocks, OD_BLOCK, 0, ctx->stream>>>(p);
+    CK(cudaGetLastError());
+    ctx->launches++;
+    if (z_out) {
+        unsigned flag = 0;
+        CK(cudaMemcpyAsync(&flag, ctx->d_red, sizeof(flag), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        *h_negative = flag ? 1 : 0;
     }
     return OD_OK;
 }

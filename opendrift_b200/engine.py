@@ -1080,6 +1080,49 @@ class Engine:
                                           C.byref(stranded)))
         return bool(stranded.value)
 
+    def plast_step(self, lon, lat, moving, z, dt, submerge=None, stokes=None, wind=None):
+        """PlastDrift.update after the current move in one launch (od_plast_step).  z: the float32 / float64 depths.
+        submerge: (K float32, terminal_velocity float32 / float64, draws float64 or None, ids int32, seed, step index) -- the new
+        depths -(K / tv * E), the quotient in tv's dtype, with E the standard exponential draws, or with draws None from the device
+        generator.
+        stokes: (us, vs, hs, xwind, ywind, hs_mode, profile, windsea_swell or None) as for stokes_drift.
+        wind: (xwind, ywind, wind_drift_factor float32 / float64, drift:wind_drift_depth).
+        Returns the new float64 depths (submerge) or None.  Raises ValueError('scale < 0'), as NumPy does, when a scale is
+        negative; the depths are then not returned (the positions have taken the Stokes and wind moves of the launch)."""
+        torch = self.torch
+        n = lon.numel()
+        assert lon.dtype == lat.dtype == torch.float64 and z.dtype in (torch.float32, torch.float64) and z.numel() == n
+        assert moving is None or moving.dtype == torch.int32
+        f32 = lambda t: t is None or (t.dtype == torch.float32 and t.numel() == n and t.is_contiguous())     # noqa: E731
+        z_out, k = None, (None,) * 6
+        if submerge is not None:
+            k = submerge
+            assert f32(k[0]) and k[0] is not None and k[1].dtype in (torch.float32, torch.float64) and k[1].numel() == n
+            assert k[2] is None or (k[2].dtype == torch.float64 and k[2].numel() == n)
+            assert k[3] is None or k[3].dtype == torch.int32
+            z_out = self.empty(n, torch.float64)
+        st, hs_mode, profile = None, 0, 0
+        if stokes is not None:
+            us, vs, hs, xw, yw, hs_mode, profile, ww = stokes
+            arrs = [us, vs, hs, xw, yw] + list(ww if ww is not None else (None,) * 6)
+            assert all(f32(t) for t in arrs)
+            st = (C.c_void_p * 11)(*[None if t is None else t.data_ptr() for t in arrs])
+            profile = self.PROFILES[profile]
+        xw = yw = wdf = None
+        wdd = 0.0
+        if wind is not None:
+            xw, yw, wdf, wdd = wind
+            assert f32(xw) and f32(yw) and wdf.dtype in (torch.float32, torch.float64) and wdf.numel() == n
+        neg = C.c_int32()
+        self._check(self.lib.od_plast_step(self.ctx, n, _ptr(lon), _ptr(lat), _ptr(moving), _ptr(z), 1 if z.dtype == torch.float64 else 0,
+                                           _ptr(z_out), _ptr(k[0]), _ptr(k[1]), int(k[1] is not None and k[1].dtype == torch.float64),
+                                           _ptr(k[2]), _ptr(k[3]), int(k[4] or 0) & (2**64 - 1), int(k[5] or 0), st, int(hs_mode),
+                                           int(profile), _ptr(xw), _ptr(yw), _ptr(wdf), int(wdf is not None and wdf.dtype == torch.float64),
+                                           float(wdd or 0.0), float(dt), C.byref(neg)))
+        if neg.value:
+            raise ValueError('scale < 0')
+        return z_out
+
     # -- particle exchange of the spatial-tile mode (od_pack_by_owner / od_unpack_records) --------------------------------------
     def pack_by_owner(self, lon, bounds, columns, want_perm=False):
         """Group the elements by the longitude strip that owns them and pack them as records (one row per element, the

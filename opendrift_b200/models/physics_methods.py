@@ -293,6 +293,21 @@ class PhysicsMethods:
             mode = 1 if any_wind else 2
         return us, vs, hs, xw, yw, mode
 
+    def _windsea_swell_arrays(self, profile):
+        """The six float32 tensors of the swell / wind-sea partition of the wave field (:418-455) for the windsea_swell profile,
+        else None; the model must have declared these variables."""
+        if profile != 'windsea_swell':
+            return None
+        env = self.environment
+        names = ('sea_surface_swell_wave_to_direction', 'sea_surface_swell_wave_peak_period_from_variance_spectral_density',
+                 'sea_surface_swell_wave_significant_height', 'sea_surface_wind_wave_to_direction',
+                 'sea_surface_wind_wave_mean_period', 'sea_surface_wind_wave_significant_height')
+        missing = [v for v in names if v not in env]
+        if missing:
+            raise AttributeError('the windsea_swell Stokes profile needs the environment variables %s '
+                                 '(add them to required_variables)' % missing)
+        return tuple(env.dev(v, self.engine) for v in names)
+
     def stokes_drift(self, factor=1, _inputs='sample'):
         """Stokes drift with a depth profile (:793-848): monochromatic / exponential / Phillips (:332-416)."""
         if not self.get_config('drift:stokes_drift', False):
@@ -303,18 +318,7 @@ class PhysicsMethods:
             return
         us, vs, hs, xw, yw, mode = inp
         eng, el, torch = self.engine, self.elements, self.engine.torch
-        ww = None
-        if profile == 'windsea_swell':
-            # the swell / wind-sea partition of the wave field (:418-455); the model must have declared these variables
-            env = self.environment
-            names = ('sea_surface_swell_wave_to_direction', 'sea_surface_swell_wave_peak_period_from_variance_spectral_density',
-                     'sea_surface_swell_wave_significant_height', 'sea_surface_wind_wave_to_direction',
-                     'sea_surface_wind_wave_mean_period', 'sea_surface_wind_wave_significant_height')
-            missing = [v for v in names if v not in env]
-            if missing:
-                raise AttributeError('the windsea_swell Stokes profile needs the environment variables %s '
-                                     '(add them to required_variables)' % missing)
-            ww = tuple(env.dev(v, eng) for v in names)
+        ww = self._windsea_swell_arrays(profile)
         if not isinstance(factor, (int, float)):
             factor = factor if isinstance(factor, torch.Tensor) else eng.to_device(np.ascontiguousarray(factor))
             if factor.dtype not in (torch.float32, torch.float64):
