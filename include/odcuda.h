@@ -501,6 +501,23 @@ int od_plast_step(od_ctx* ctx, int64_t n, double* d_lon, double* d_lat, const in
                   const float* d_xwind, const float* d_ywind, const void* d_wdf, int32_t wdf_f64, double wind_drift_depth, double dt,
                   int32_t* h_negative);
 
+/* ---- LarvalFish ----------------------------------------------------------------------------------------
+ * od_larval_develop: LarvalFish.update_fish_larvae and update_terminal_velocity (models/larvalfish.py) for n elements in one
+ * launch (csrc/od_larval.cuh).  d_t, d_s: float32 sea_water_temperature and sea_water_salinity.  Each element array is float32 or
+ * float64 by its *_f64 flag; hatched is uint8 or float64.
+ *   develop != 0: hatching (stage_fraction, hatched), growth (weight) and length, in place.
+ *   d_w_out != NULL: the terminal velocity of every element, float64 if diameter_f64 || nbs_f64, else float32.
+ *   h_flags != NULL: OR of LARVAL_STAGED (1: some element is an egg or a larva), LARVAL_HOT (2: some T > 100) and
+ *   LARVAL_NAN_T (4: some T is NaN) (synchronises); NULL: no read-back.
+ * od_larval_migrate: larvae_vertical_migration: every element with hatched == 1 gets
+ *   z = min(0, z + direction * fraction * swim(length) * dt), z float32 or float64 (z_f64). */
+int od_larval_develop(od_ctx* ctx, int64_t n, const float* d_t, const float* d_s, void* d_hatched, int32_t hatched_f64,
+                      void* d_stage, int32_t stage_f64, void* d_weight, int32_t weight_f64, void* d_length, int32_t length_f64,
+                      const void* d_diameter, int32_t diameter_f64, const void* d_nbs, int32_t nbs_f64, int32_t develop,
+                      void* d_w_out, double dt, int32_t* h_flags);
+int od_larval_migrate(od_ctx* ctx, int64_t n, const void* d_hatched, int32_t hatched_f64, const void* d_length, int32_t length_f64,
+                      void* d_z, int32_t z_f64, double fraction, double direction, double dt);
+
 /* ---- analytical readers on a projected plane ---------------------------------------------------------
  * BASELINE configs[0]: opendrift/readers/reader_double_gyre.py (a ContinuousReader, basereader/continuous.py:9-48) on the
  * spherical stereographic plane its constructor asks pyproj for (reader_double_gyre.py:27-31).  The reader chain of

@@ -208,6 +208,9 @@ SYMBOLS = {
                                C.c_int32, C.c_float, C.c_int32, C.c_double, C.POINTER(C.c_int32)]),
     'od_plast_step': (C.c_int, [_P, C.c_int64, _P, _P, _P, _P, C.c_int32, _P, _P, _P, C.c_int32, _P, _P, C.c_uint64, C.c_int32, _P, C.c_int32,
                                 C.c_int32, _P, _P, _P, C.c_int32, C.c_double, C.c_double, C.POINTER(C.c_int32)]),
+    'od_larval_develop': (C.c_int, [_P, C.c_int64, _P, _P, _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, _P,
+                                    C.c_int32, C.c_int32, _P, C.c_double, C.POINTER(C.c_int32)]),
+    'od_larval_migrate': (C.c_int, [_P, C.c_int64, _P, C.c_int32, _P, C.c_int32, _P, C.c_int32, C.c_double, C.c_double, C.c_double]),
     'od_vertical_buoyancy': (C.c_int, [_P, C.POINTER(BuoyancyArgs)]),
     'od_bookkeeping': (C.c_int, [_P, C.POINTER(BookkeepArgs)]),
     'od_coastline': (C.c_int, [_P, C.POINTER(CoastArgs)]),

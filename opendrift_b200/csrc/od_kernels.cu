@@ -22,6 +22,7 @@
 #include "od_leeway.cuh"
 #include "od_ship.cuh"
 #include "od_plast.cuh"
+#include "od_larval.cuh"
 #include "od_analytic.cuh"
 #include "od_history.cuh"
 #include "od_bookkeep.cuh"
@@ -714,6 +715,22 @@ __global__ void __launch_bounds__(256) ship_kernel(const ShipParams p) {
 __global__ void __launch_bounds__(OD_BLOCK) plast_kernel(const PlastParams p) {
     for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += (int64_t)gridDim.x * blockDim.x)
         plast_particle(p, i);
+}
+
+// ---- LarvalFish ----------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(OD_BLOCK) larval_develop_kernel(const LarvalParams p, unsigned* flags) {
+    unsigned acc = 0;
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += (int64_t)gridDim.x * blockDim.x)
+        acc |= larval_develop_one(p, i);
+    if (flags) {
+        acc = __reduce_or_sync(0xffffffffu, acc);
+        if (acc && (threadIdx.x & 31) == 0) atomicOr(flags, acc);
+    }
+}
+
+__global__ void __launch_bounds__(OD_BLOCK) larval_migrate_kernel(const LarvalParams p) {
+    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += (int64_t)gridDim.x * blockDim.x)
+        larval_migrate_one(p, i);
 }
 
 // ---- Leeway -------------------------------------------------------------------------------------------
@@ -1930,6 +1947,59 @@ extern "C" int od_plast_step(od_ctx* ctx, int64_t n, double* lon, double* lat, c
         CK(cudaStreamSynchronize(ctx->stream));
         *h_negative = flag ? 1 : 0;
     }
+    return OD_OK;
+}
+
+extern "C" int od_larval_develop(od_ctx* ctx, int64_t n, const float* t, const float* s, void* hatched, int32_t hatched_f64,
+                                 void* stage, int32_t stage_f64, void* weight, int32_t weight_f64, void* length, int32_t length_f64,
+                                 const void* diameter, int32_t diameter_f64, const void* nbs, int32_t nbs_f64, int32_t develop,
+                                 void* w_out, double dt, int32_t* h_flags) {
+    if (!ctx || n < 0) return fail(ctx, OD_ERR_ARG, "od_larval_develop: bad arguments");
+    if (h_flags) *h_flags = 0;
+    if (n == 0) return OD_OK;
+    if (!t || (develop && (!hatched || !stage || !weight || !length)) || (w_out && (!s || !diameter || !nbs)))
+        return fail(ctx, OD_ERR_ARG, "od_larval_develop: bad arguments");
+    CK(cudaSetDevice(ctx->device));
+    LarvalParams p;
+    memset(&p, 0, sizeof(p));
+    p.n = n; p.t = t; p.s = s; p.hatched = hatched; p.stage = stage; p.weight = weight; p.length = length;
+    p.diameter = diameter; p.nbs = nbs; p.w_out = w_out; p.develop = develop; p.dt = dt;
+    p.hatched_f64 = hatched_f64; p.stage_f64 = stage_f64; p.weight_f64 = weight_f64; p.length_f64 = length_f64;
+    p.diameter_f64 = diameter_f64; p.nbs_f64 = nbs_f64;
+    unsigned* flags = nullptr;
+    if (h_flags) {
+        if (!ctx->d_red) CK(cudaMalloc(&ctx->d_red, 2 * sizeof(unsigned)));
+        CK(cudaMemsetAsync(ctx->d_red, 0, sizeof(unsigned), ctx->stream));
+        flags = ctx->d_red;
+    }
+    int64_t blocks = (n + OD_BLOCK - 1) / OD_BLOCK;
+    if (blocks > (int64_t)ctx->sm_count * 8) blocks = (int64_t)ctx->sm_count * 8;
+    larval_develop_kernel<<<(unsigned)blocks, OD_BLOCK, 0, ctx->stream>>>(p, flags);
+    CK(cudaGetLastError());
+    ctx->launches++;
+    if (h_flags) {
+        unsigned f = 0;
+        CK(cudaMemcpyAsync(&f, ctx->d_red, sizeof(f), cudaMemcpyDeviceToHost, ctx->stream));
+        CK(cudaStreamSynchronize(ctx->stream));
+        *h_flags = (int32_t)f;
+    }
+    return OD_OK;
+}
+
+extern "C" int od_larval_migrate(od_ctx* ctx, int64_t n, const void* hatched, int32_t hatched_f64, const void* length,
+                                 int32_t length_f64, void* z, int32_t z_f64, double fraction, double direction, double dt) {
+    if (!ctx || n < 0 || (n > 0 && (!hatched || !length || !z))) return fail(ctx, OD_ERR_ARG, "od_larval_migrate: bad arguments");
+    if (n == 0) return OD_OK;
+    CK(cudaSetDevice(ctx->device));
+    LarvalParams p;
+    memset(&p, 0, sizeof(p));
+    p.n = n; p.hatched = (void*)hatched; p.hatched_f64 = hatched_f64; p.length = (void*)length; p.length_f64 = length_f64;
+    p.z = z; p.z_f64 = z_f64; p.swim = fraction; p.dir = direction; p.dt = dt;
+    int64_t blocks = (n + OD_BLOCK - 1) / OD_BLOCK;
+    if (blocks > (int64_t)ctx->sm_count * 8) blocks = (int64_t)ctx->sm_count * 8;
+    larval_migrate_kernel<<<(unsigned)blocks, OD_BLOCK, 0, ctx->stream>>>(p);
+    CK(cudaGetLastError());
+    ctx->launches++;
     return OD_OK;
 }
 

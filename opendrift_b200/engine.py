@@ -1123,6 +1123,45 @@ class Engine:
             raise ValueError('scale < 0')
         return z_out
 
+    LARVAL_STAGED, LARVAL_HOT, LARVAL_NAN_T = 1, 2, 4
+
+    def larval_develop(self, t, s, el, dt, develop=True, velocity=True, flags=True):
+        """LarvalFish's hatching, growth and length (develop) and terminal velocity (velocity) in one launch (od_larval_develop).
+        t, s: float32 temperature and salinity; el: dict of the element tensors hatched (uint8 / float64), stage_fraction, weight,
+        length, diameter, neutral_buoyancy_salinity (float32 / float64), updated in place.  Returns (W or None, flags or None):
+        W the new terminal velocity tensor (float64 if diameter or neutral_buoyancy_salinity is), flags the OR of LARVAL_STAGED,
+        LARVAL_HOT and LARVAL_NAN_T over the elements (a 4-byte read-back) when flags is True."""
+        torch = self.torch
+        n = t.numel()
+        fl = lambda x: (x.dtype in (torch.float32, torch.float64) and x.numel() == n and x.is_contiguous())     # noqa: E731
+        f64 = lambda x: int(x is not None and x.dtype == torch.float64)                                        # noqa: E731
+        assert t.dtype == torch.float32 and t.is_contiguous()
+        h = sf = w = ln = d = sal = w_out = None
+        if develop:
+            h, sf, w, ln = el['hatched'], el['stage_fraction'], el['weight'], el['length']
+            assert h.dtype in (torch.uint8, torch.float64) and h.numel() == n and h.is_contiguous()
+            assert fl(sf) and fl(w) and fl(ln)
+        if velocity:
+            d, sal = el['diameter'], el['neutral_buoyancy_salinity']
+            assert s.dtype == torch.float32 and s.is_contiguous() and fl(d) and fl(sal)
+            w_out = self.empty(n, torch.float64 if (f64(d) or f64(sal)) else torch.float32)
+        out = C.c_int32()
+        self._check(self.lib.od_larval_develop(self.ctx, n, _ptr(t), _ptr(s), _ptr(h), f64(h), _ptr(sf), f64(sf), _ptr(w), f64(w),
+                                               _ptr(ln), f64(ln), _ptr(d), f64(d), _ptr(sal), f64(sal), int(bool(develop)), _ptr(w_out),
+                                               float(dt), C.byref(out) if flags else None))
+        return w_out, (out.value if flags else None)
+
+    def larval_migrate(self, hatched, length, z, fraction, direction, dt):
+        """LarvalFish's larvae_vertical_migration in one launch (od_larval_migrate): z (float32 / float64) in place."""
+        torch = self.torch
+        n = z.numel()
+        assert hatched.dtype in (torch.uint8, torch.float64) and hatched.numel() == n and hatched.is_contiguous()
+        assert length.dtype in (torch.float32, torch.float64) and length.numel() == n and length.is_contiguous()
+        assert z.dtype in (torch.float32, torch.float64) and z.is_contiguous()
+        self._check(self.lib.od_larval_migrate(self.ctx, n, _ptr(hatched), int(hatched.dtype == torch.float64), _ptr(length),
+                                               int(length.dtype == torch.float64), _ptr(z), int(z.dtype == torch.float64),
+                                               float(fraction), float(direction), float(dt)))
+
     # -- particle exchange of the spatial-tile mode (od_pack_by_owner / od_unpack_records) --------------------------------------
     def pack_by_owner(self, lon, bounds, columns, want_perm=False):
         """Group the elements by the longitude strip that owns them and pack them as records (one row per element, the

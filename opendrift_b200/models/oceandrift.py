@@ -230,7 +230,13 @@ class OceanDrift(OpenDriftSimulation):
             if len(self.env.readers_for('ocean_vertical_diffusivity', self.time)) > 1:
                 raise NotImplementedError('vertical mixing on the GPU path takes its diffusivity profile from one reader; '
                                           'several readers provide ocean_vertical_diffusivity at %s' % self.time)
-            if r is not None and hasattr(r, 'group_of'):
+            kc = self._constant_reader_diffusivity()
+            if kc is not None:
+                # a constant reader's profile is that float32 value at every level (gradient 0): the constant model with it,
+                # or Large et al. (1994) when it equals the fallback, as the reference decides (:430-435)
+                fb = self.env.fallback('ocean_vertical_diffusivity')
+                model = 'windspeed_Large1994' if fb is not None and np.float32(kc) == np.float32(fb) else 'constant'
+            elif r is not None and hasattr(r, 'group_of'):
                 g, _ = r.group_of('ocean_vertical_diffusivity')
             else:
                 model = 'windspeed_Large1994'
@@ -243,13 +249,24 @@ class OceanDrift(OpenDriftSimulation):
             floor = self.environment.dev('sea_floor_depth_below_sea_level', self.engine)
         return g, model, dt_mix, ntimes, floor
 
+    def _constant_reader_diffusivity(self):
+        """With vertical_mixing:diffusivitymodel = 'environment': the float32 value a constant reader (readers/reader_constant.py)
+        gives for ocean_vertical_diffusivity at this time, else None."""
+        from ..readers import reader_constant
+        if self.get_config('vertical_mixing:diffusivitymodel') != 'environment':
+            return None
+        r = self.env.reader_for('ocean_vertical_diffusivity', self.time)
+        if not isinstance(r, reader_constant.Reader):
+            return None
+        return float(np.float32(r._parameter_value_map['ocean_vertical_diffusivity'][0]))
+
     def _mixing_reads_environment(self):
         """True when the mixing launch needs start-of-step environment samples (wind for the analytical diffusivity models, a
         mixed-layer or sea-floor depth that comes from a reader) in addition to the diffusivity profile itself."""
         model = self.get_config('vertical_mixing:diffusivitymodel')
         if model == 'environment':
             r = self.env.reader_for('ocean_vertical_diffusivity', self.time)
-            if r is None or not hasattr(r, 'group_of'):
+            if r is None or not hasattr(r, 'group_of') or self._constant_reader_diffusivity() is not None:
                 return True                           # falls back to Large et al. (1994): wind speed
         else:
             return True
@@ -264,6 +281,15 @@ class OceanDrift(OpenDriftSimulation):
             fb = self.env.fallback(var)
             return float(default if fb is None else fb)
         return self.environment.dev(var, self.engine)
+
+    def _env_f32(self, name):
+        """The step's float32 environment tensor of `name`, contiguous (kept in the environment)."""
+        torch = self.engine.torch
+        t = self.environment.dev(name, self.engine)
+        if t.dtype != torch.float32 or not t.is_contiguous():
+            t = t.to(torch.float32).contiguous()
+            self.environment.set_dev(name, t)
+        return t
 
     def _mix(self, lon0, lat0, z_in, pos_f32):
         """Run the mixing kernel from start-of-step positions; returns the new float64 depth tensor."""
@@ -295,6 +321,7 @@ class OceanDrift(OpenDriftSimulation):
         if ids.dtype != torch.int32:
             ids = ids.to(torch.int32)
         kw = {}
+        kc = self._constant_reader_diffusivity()
         if model != 'environment':
             env = self.environment
             if 'x_wind' in env and 'y_wind' in env:
@@ -305,7 +332,7 @@ class OceanDrift(OpenDriftSimulation):
             kw = dict(model=model, wind_speed=ws,
                       mld=self._env_scalar_or_tensor('ocean_mixed_layer_thickness', 50.0),
                       background=self.get_config('vertical_mixing:background_diffusivity'),
-                      k_const=float(self.env.fallback('ocean_vertical_diffusivity') or 0.0))
+                      k_const=kc if kc is not None else float(self.env.fallback('ocean_vertical_diffusivity') or 0.0))
         # 'Let particles stick to bottom' (oceandrift.py:559-564) only acts when a reader provides the sea floor
         action, code, status = 0, 0, None
         if self.env.priority_list.get('sea_floor_depth_below_sea_level'):

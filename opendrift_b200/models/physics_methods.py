@@ -5,7 +5,33 @@ start-of-step environment is the one sampled by the run loop (self.environment).
 import numpy as np
 
 
+def seawater_dynamic_viscosity(T, S, model='sharqawy'):
+    """Dynamic viscosity of sea water in Pa s (:139-178), NumPy on host arrays: Sharqawy et al. (2010) for T in degrees Celsius
+    and S in g/kg, or with model='ladim' the linear fit of the LADIM code."""
+    if model == 'ladim':
+        return 0.001 * (1.7915 - 0.0538 * T + 0.0007 * (T ** (2.0)) + 0.0023 * S)
+    if model != 'sharqawy':
+        raise ValueError(f'Model {model} not available')
+    mu_pure = 4.2844e-5 + 1.0 / (0.157 * (T + 64.993) ** 2 - 91.296)
+    a = 1.541 + 1.998e-2 * T - 9.52e-5 * T ** 2
+    b = 7.974 - 7.561e-2 * T + 4.724e-4 * T ** 2
+    return mu_pure * (1 + a * (S / 1000) + b * (S / 1000) ** 2)
+
+
 class PhysicsMethods:
+
+    @staticmethod
+    def sea_water_density(T=10., S=35.):
+        """Density of sea water at one atmosphere (:574-609; Fofonoff and Millard 1983, UNESCO technical papers in marine science
+        44), NumPy on host arrays: T in degrees Celsius, S in PSU.  Raises ValueError when the largest T exceeds 100."""
+        if np.atleast_1d(T).max() > 100:
+            raise ValueError('Temperature should be in celcius, but is > 100')
+        # pure water (Bigg 1967), then the salinity terms
+        r1 = ((((6.536332E-09 * T - 1.120083E-06) * T + 1.001685E-04) * T - 9.095290E-03) * T + 6.793952E-02) * T - 28.263737
+        r2 = (((5.3875E-09 * T - 8.2467E-07) * T + 7.6438E-05) * T - 4.0899E-03) * T + 8.24493E-01
+        r3 = (-1.6546E-06 * T + 1.0227E-04) * T - 5.72466E-03
+        sigma = r1 + (4.8314E-04 * S + r3 * np.sqrt(S) + r2) * S
+        return sigma + 28.106331 + 1000.
 
     def _current_group(self, t):
         # the first reader that covers any stage time of the step that starts at t (a reader whose coverage begins inside

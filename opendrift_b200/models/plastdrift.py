@@ -100,15 +100,6 @@ class PlastDrift(OceanDrift):
             wind = (self._env_f32('x_wind'), self._env_f32('y_wind'), self.get_config('drift:wind_drift_depth', 0) or 0)
         self._launch(submerge=mixing and model == 'analytical', stokes=stokes, wind=wind)
 
-    def _env_f32(self, name):
-        """The step's float32 environment tensor of `name`, contiguous (kept in the environment)."""
-        torch = self.engine.torch
-        t = self.environment.dev(name, self.engine)
-        if t.dtype != torch.float32 or not t.is_contiguous():
-            t = t.to(torch.float32).contiguous()
-            self.environment.set_dev(name, t)
-        return t
-
     def _launch(self, submerge, stokes, wind):
         eng, el, torch = self.engine, self.elements, self.engine.torch
         n = len(el)
