@@ -159,6 +159,11 @@ int od_group_fill_nan(od_ctx* ctx, int group, int slot, int comp, int max_iterat
 int od_group_slot_ptr(od_ctx* ctx, int group, int slot, int comp, float** d_out);
 /* tell the library a slot's contents changed behind its back (after a broadcast into od_group_slot_ptr) */
 int od_group_touch(od_ctx* ctx, int group, int slot);
+/* Build the pair texels of the slabs in slots (slot_a, slot_b) now, on the current stream, ahead of the first launch that
+ * samples between them (e.g. on the copy stream right after the later slab was put into its slot).  The cache entry the
+ * launches used last is never overwritten; a launch that samples the pair orders its stream behind the build.  No-op when
+ * the pair is cached already. */
+int od_group_prepare_pair(od_ctx* ctx, int group, int slot_a, int slot_b);
 /* Sub-block readers: the blocks a reader hands out cover the elements plus a buffer (StructuredReader block cache,
  * readers/basereader/structured.py:243-318; block supplier readers/reader_netCDF_CF_generic.py:404-626).  The group keeps the slots
  * it was defined with (capacity = its full grid); this call replaces nx, ny and the block-relative index geometry (the block's own

@@ -184,6 +184,7 @@ SYMBOLS = {
     'od_group_fill_nan': (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int64)]),
     'od_group_slot_ptr': (C.c_int, [_P, C.c_int, C.c_int, C.c_int, C.POINTER(_P)]),
     'od_group_touch': (C.c_int, [_P, C.c_int, C.c_int]),
+    'od_group_prepare_pair': (C.c_int, [_P, C.c_int, C.c_int, C.c_int]),
     'od_group_set_fallback': (C.c_int, [_P, C.c_int, C.c_float, C.c_float]),
     'od_group_set_window': (C.c_int, [_P, C.c_int, C.POINTER(GroupDesc)]),
     'od_bbox': (C.c_int, [_P, C.c_int64, _P, _P, C.POINTER(C.c_double)]),

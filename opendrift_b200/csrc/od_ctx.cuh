@@ -46,6 +46,10 @@ struct PairEntry {
     int slot_a = -1, slot_b = -1;
     uint64_t ver_a = 0, ver_b = 0;
     uint64_t last_use = 0;
+    // built ahead on another stream (od_group_prepare_pair): `ready` marks the end of the build, and a launch that reads or
+    // rebuilds the entry orders its stream behind it while `pending` is set
+    cudaEvent_t ready = nullptr;
+    bool pending = false;
 };
 
 struct Group {

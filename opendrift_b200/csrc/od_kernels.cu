@@ -57,6 +57,7 @@ static void free_group(Group& g) {
     g.h_levels.clear();
     for (auto& p : g.pairs) {
         if (p.tex) cudaFree(p.tex);
+        if (p.ready) cudaEventDestroy(p.ready);
         p = PairEntry();
     }
     g.defined = false;
@@ -453,44 +454,22 @@ static bool make_tensor_map(const Group& g, float* tex, CUtensorMap* out) {
                CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// Resolve a time sample to pair texels (building / reusing a cached pair).
-static int resolve_pair(od_ctx* ctx, int group, const od_time_sample& ts, PairRef* out) {
-    Group& g = ctx->groups[group];
-    const int nc = g.desc.ncomp;
-    if (ts.mode == OD_T_MISSING) {
-        out->tex = nullptr; out->mode = OD_T_MISSING; out->pad_ = 0; out->w = 0.0;
+// A cached pair is about to be read or overwritten on ctx->stream: order the stream behind its build when that ran ahead on
+// another stream (od_group_prepare_pair) and may not have finished.
+static int order_after_build(od_ctx* ctx, PairEntry& p) {
+    if (!p.pending) return OD_OK;
+    if (cudaEventQuery(p.ready) == cudaSuccess) {
+        p.pending = false;
         return OD_OK;
     }
-    int sa = ts.slot_a, sb = ts.slot_b;
-    if (ts.mode == OD_T_FIRST) sb = (sb < 0 || sb >= g.desc.n_slots) ? sa : sb;
-    if (ts.mode == OD_T_SECOND) sa = (sa < 0 || sa >= g.desc.n_slots) ? sb : sa;
-    if (sa < 0 || sa >= g.desc.n_slots || sb < 0 || sb >= g.desc.n_slots || ts.mode < 0 || ts.mode > 2)
-        return fail(ctx, OD_ERR_ARG, "bad time sample");
-    out->w = ts.w;
-    out->pad_ = 0;
-    // a single-slab sample can be served by any cached pair that contains the slab
-    if (ts.mode != OD_T_LERP) {
-        const int need = ts.mode == OD_T_FIRST ? sa : sb;
-        for (auto& p : g.pairs) {
-            if (!p.tex) continue;
-            if (p.slot_a == need && p.ver_a == g.version[need]) { out->tex = p.tex; out->mode = OD_T_FIRST; p.last_use = ++ctx->tick; return OD_OK; }
-            if (p.slot_b == need && p.ver_b == g.version[need]) { out->tex = p.tex; out->mode = OD_T_SECOND; p.last_use = ++ctx->tick; return OD_OK; }
-        }
-    }
-    for (auto& p : g.pairs) {
-        if (p.tex && p.slot_a == sa && p.slot_b == sb && p.ver_a == g.version[sa] && p.ver_b == g.version[sb]) {
-            out->tex = p.tex;
-            out->mode = ts.mode;
-            p.last_use = ++ctx->tick;
-            return OD_OK;
-        }
-    }
-    // build into the least recently used entry
-    PairEntry* victim = &g.pairs[0];
-    for (auto& p : g.pairs) {
-        if (!p.tex) { victim = &p; break; }
-        if (p.last_use < victim->last_use) victim = &p;
-    }
+    cudaGetLastError();                              // (cudaErrorNotReady is not an error)
+    CK(cudaStreamWaitEvent(ctx->stream, p.ready, 0));
+    return OD_OK;
+}
+
+// Pack slabs sa, sb of group g into the cache entry `victim` on ctx->stream, with at most `max_blocks` thread blocks.
+static int build_pair(od_ctx* ctx, Group& g, int sa, int sb, PairEntry* victim, int max_blocks) {
+    const int nc = g.desc.ncomp;
     if (!victim->tex) {
         // first pair of this group: allocate the whole cache now, so that no later step pays for a cudaMalloc
         // (tens of milliseconds for a 200 MB block on a cold device, and an implicit device synchronisation)
@@ -507,10 +486,12 @@ static int resolve_pair(od_ctx* ctx, int group, const od_time_sample& ts, PairRe
             p.tmap_ok = make_tensor_map(g, p.tex, &p.tmap);
         }
     }
+    int rc = order_after_build(ctx, *victim);
+    if (rc) return rc;
+    victim->pending = false;
     const int64_t cells = (int64_t)g.cells();
     int blocks = (int)((cells + OD_BLOCK - 1) / OD_BLOCK);
-    const int cap = ctx->sm_count * 8;
-    if (blocks > cap) blocks = cap;
+    if (blocks > max_blocks) blocks = max_blocks;
     if (nc == 2)
         pack_pair2_kernel<<<blocks, OD_BLOCK, 0, ctx->stream>>>(g.slots[(size_t)sa * 2], g.slots[(size_t)sa * 2 + 1],
                                                                 g.slots[(size_t)sb * 2], g.slots[(size_t)sb * 2 + 1],
@@ -524,6 +505,93 @@ static int resolve_pair(od_ctx* ctx, int group, const od_time_sample& ts, PairRe
     victim->ver_a = g.version[sa];
     victim->ver_b = g.version[sb];
     victim->last_use = ++ctx->tick;
+    return OD_OK;
+}
+
+// Build the pair texels of slots (slot_a, slot_b) ahead of their first use, on the current stream (the copy stream that has
+// just put one of the two slabs into its slot).  The entry the launches use most recently is never overwritten; the build
+// records an event that resolve_pair orders the using stream behind.  A pair that is cached already costs nothing.
+extern "C" int od_group_prepare_pair(od_ctx* ctx, int group, int slot_a, int slot_b) {
+    int rc = check_slot(ctx, group, slot_a, 0);
+    if (rc) return rc;
+    rc = check_slot(ctx, group, slot_b, 0);
+    if (rc) return rc;
+    CK(cudaSetDevice(ctx->device));
+    Group& g = ctx->groups[group];
+    PairEntry* newest = nullptr;
+    for (auto& p : g.pairs) {
+        if (p.tex && p.slot_a == slot_a && p.slot_b == slot_b && p.ver_a == g.version[slot_a] && p.ver_b == g.version[slot_b])
+            return OD_OK;
+        if (p.tex && (!newest || p.last_use > newest->last_use)) newest = &p;
+    }
+    PairEntry* victim = nullptr;
+    for (auto& p : g.pairs) {
+        if (&p == newest) continue;
+        if (!p.tex) { victim = &p; break; }
+        if (!victim || p.last_use < victim->last_use) victim = &p;
+    }
+    if (!victim) return OD_OK;                       // a one-entry cache: the pair is built when it is first needed
+    // One thread block per SM: the build fits beside the step kernel's blocks and has a reader hour to finish, so it takes
+    // memory bandwidth the issue-bound step leaves over rather than SM slots from it.
+    rc = build_pair(ctx, g, slot_a, slot_b, victim, ctx->sm_count);
+    if (rc) return rc;
+    if (!victim->ready) CK(cudaEventCreateWithFlags(&victim->ready, cudaEventDisableTiming));
+    CK(cudaEventRecord(victim->ready, ctx->stream));
+    victim->pending = true;
+    return OD_OK;
+}
+
+// Resolve a time sample to pair texels (building / reusing a cached pair).
+static int resolve_pair(od_ctx* ctx, int group, const od_time_sample& ts, PairRef* out) {
+    Group& g = ctx->groups[group];
+    if (ts.mode == OD_T_MISSING) {
+        out->tex = nullptr; out->mode = OD_T_MISSING; out->pad_ = 0; out->w = 0.0;
+        return OD_OK;
+    }
+    int sa = ts.slot_a, sb = ts.slot_b;
+    if (ts.mode == OD_T_FIRST) sb = (sb < 0 || sb >= g.desc.n_slots) ? sa : sb;
+    if (ts.mode == OD_T_SECOND) sa = (sa < 0 || sa >= g.desc.n_slots) ? sb : sa;
+    if (sa < 0 || sa >= g.desc.n_slots || sb < 0 || sb >= g.desc.n_slots || ts.mode < 0 || ts.mode > 2)
+        return fail(ctx, OD_ERR_ARG, "bad time sample");
+    out->w = ts.w;
+    out->pad_ = 0;
+    // a single-slab sample can be served by any cached pair that contains the slab; one whose build ahead is still running is
+    // taken only when no other pair has the slab
+    if (ts.mode != OD_T_LERP) {
+        const int need = ts.mode == OD_T_FIRST ? sa : sb;
+        for (int pass = 0; pass < 2; ++pass) {
+            for (auto& p : g.pairs) {
+                if (!p.tex) continue;
+                if (pass == 0 && p.pending && cudaEventQuery(p.ready) != cudaSuccess) { cudaGetLastError(); continue; }
+                int mode = -1;
+                if (p.slot_a == need && p.ver_a == g.version[need]) mode = OD_T_FIRST;
+                else if (p.slot_b == need && p.ver_b == g.version[need]) mode = OD_T_SECOND;
+                if (mode < 0) continue;
+                const int rc = order_after_build(ctx, p);
+                if (rc) return rc;
+                out->tex = p.tex; out->mode = mode; p.last_use = ++ctx->tick;
+                return OD_OK;
+            }
+        }
+    }
+    for (auto& p : g.pairs) {
+        if (p.tex && p.slot_a == sa && p.slot_b == sb && p.ver_a == g.version[sa] && p.ver_b == g.version[sb]) {
+            const int rc = order_after_build(ctx, p);
+            if (rc) return rc;
+            out->tex = p.tex;
+            out->mode = ts.mode;
+            p.last_use = ++ctx->tick;
+            return OD_OK;
+        }
+    }
+    // build into the least recently used entry
+    PairEntry* victim = &g.pairs[0];
+    for (auto& p : g.pairs) {
+        if (!p.tex) { victim = &p; break; }
+        if (p.last_use < victim->last_use) victim = &p;
+    }
+    const int rc = build_pair(ctx, g, sa, sb, victim, ctx->sm_count * 8);
+    if (rc) return rc;
     out->tex = victim->tex;
     out->mode = ts.mode;
     return OD_OK;
@@ -802,16 +870,20 @@ __global__ void __launch_bounds__(OD_BLOCK) cell_key_kernel(const SortParams p, 
     if (p.g.nz > 1) load_levels(lv, p.g);
     __syncthreads();
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= p.n) return;
-    const HorizW h = PROJ ? horiz_weights_h(p.g, p.lon[i], p.lat[i], false) : horiz_weights(p.g, p.lon[i], p.lat[i], false);
-    int key = 0;
-    if (h.valid) {
-        const int iy = h.i00 / p.g.nx, ix = h.i00 - iy * p.g.nx;
-        const VertW vw = vert_weights(p.g, (const double*)lv.zs, (const double*)lv.zy, (p.z && p.g.nz > 1) ? (double)p.z[i] : 0.0);
-        key = 1 + (vw.ia * p.nty + iy / p.tile) * p.ntx + ix / p.tile;
+    int key = -1;                                    // (lanes past the end: a group of their own, no count)
+    if (i < p.n) {
+        const HorizW h = PROJ ? horiz_weights_h(p.g, p.lon[i], p.lat[i], false) : horiz_weights(p.g, p.lon[i], p.lat[i], false);
+        key = 0;
+        if (h.valid) {
+            const int iy = h.i00 / p.g.nx, ix = h.i00 - iy * p.g.nx;
+            const VertW vw = vert_weights(p.g, (const double*)lv.zs, (const double*)lv.zy, (p.z && p.g.nz > 1) ? (double)p.z[i] : 0.0);
+            key = 1 + (vw.ia * p.nty + iy / p.tile) * p.ntx + ix / p.tile;
+        }
+        keys[i] = key;
     }
-    keys[i] = key;
-    atomicAdd(&bins[key], 1);
+    // cell-sorted particles: the lanes of a warp mostly share one to three bins; one atomic per bin and warp
+    const unsigned peers = __match_any_sync(0xffffffffu, key);
+    if (key >= 0 && (threadIdx.x & 31) == __ffs(peers) - 1) atomicAdd(&bins[key], __popc(peers));
 }
 
 // exclusive scan of the bin counts, one block (bins <= a few hundred thousand)
@@ -911,9 +983,14 @@ static int scan_exclusive(od_ctx* ctx, int32_t* bins, int nbins) {
 __global__ void __launch_bounds__(OD_BLOCK) scatter_perm_kernel(int64_t n, const int32_t* __restrict__ keys,
                                                                  int32_t* __restrict__ bins, int32_t* __restrict__ perm) {
     const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= n) return;
-    const int pos = atomicAdd(&bins[keys[i]], 1);
-    perm[pos] = (int32_t)i;
+    const int key = i < n ? keys[i] : -1;
+    // the lanes of a warp that share a bin take consecutive places of it: the first of them reserves the group's range
+    const unsigned peers = __match_any_sync(0xffffffffu, key);
+    const int lane = threadIdx.x & 31, leader = __ffs(peers) - 1;
+    int base = 0;
+    if (key >= 0 && lane == leader) base = atomicAdd(&bins[key], __popc(peers));
+    base = __shfl_sync(0xffffffffu, base, leader);
+    if (key >= 0) perm[base + __popc(peers & ((1u << lane) - 1u))] = (int32_t)i;
 }
 
 // ---- stable partition (deactivated-element compaction) ---------------------------------------------------

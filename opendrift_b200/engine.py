@@ -129,6 +129,7 @@ class FieldGroup:
         self.use = [0] * n_slots
         self.ready = [None] * n_slots     # event of a slab that was put into its slot on the copy stream (prefetch), until first use
         self.prefetch_on = True
+        self.ahead_pair = None            # (slot_a, slot_b) whose pair texels the copy stream builds after a prefetch
         self._tick = 0
         d = GroupDesc()
         d.ncomp, d.nx, d.ny = ncomp, len(self.lon), len(self.lat)
@@ -244,6 +245,11 @@ class FieldGroup:
             return False
         try:
             self._load(ti, s)
+            # the pair texels the run samples next (this slab and its neighbour towards the run's current pair): end_copy_stream
+            # builds them on the copy stream, rather than the first step that needs them on the compute stream
+            nb = ti - 1 if eng.direction >= 0 else ti + 1
+            if nb in self.resident:
+                self.ahead_pair = (self.resident.index(nb), s) if nb < ti else (s, self.resident.index(nb))
             self.ready[s] = eng.end_copy_stream()
         except Exception:
             eng.end_copy_stream()
@@ -472,7 +478,13 @@ class Engine:
         return True
 
     def end_copy_stream(self):
-        """Back to the compute stream; returns an event that marks the end of what was queued on the copy stream."""
+        """Back to the compute stream; returns an event that marks the end of what was queued on the copy stream, which
+        includes the pair texels of the groups' `ahead_pair` (od_group_prepare_pair)."""
+        for g in list(self.groups.values()):
+            if g.ahead_pair is not None:
+                sa, sb = g.ahead_pair
+                g.ahead_pair = None
+                self._check(self.lib.od_group_prepare_pair(self.ctx, g.gid, sa, sb))
         ev = self.torch.cuda.Event()
         ev.record(self._copy_stream)
         self._ctx_mgr.__exit__(None, None, None)
